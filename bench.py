@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — baseline-visibilities/s through predict+Jacobian (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            (own arm, hand-written sm_100a kernels)
+  python bench.py --gpus N --steps K --warmup W            (own arm, hand-written sm_90a kernels)
   python bench.py --impl reference --gpus N --steps K ...  (the reference's CPU path, bounded sample)
 
 One "step" = one complete direction-dependent solve of the workload on device-resident inputs:
@@ -70,7 +70,19 @@ def parse():
                          "workload it discards every visit (DESIGN.md 9b)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned to its caller "
+                         "(solved Jones, and retval / mean nu / res_0 / res_1) as DIR/<workload>_*.npy.  "
+                         "The inputs of C4 / C4rtr / C5 and --devgen (coherencies, and the data as a "
+                         "prediction of the true Jones plus seeded noise) are made by this library's "
+                         "own device kernels, so builds that change those kernels get different inputs; "
+                         "the 62-station workloads' inputs come from the host generator alone")
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs dumps what the library computed; it does not apply to --impl reference")
+    return args
 
 
 def solve_args(name):
@@ -127,7 +139,7 @@ def workload_shape(name):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons during the timed region"""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -185,20 +197,7 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(workload="C2"):
-    """dram bytes per launch of the dominant kernel from the committed ncu --set full capture"""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            t = json.load(f)
-        if workload in ("C3rtr", "C3nsd"):
-            return t.get("k_rtr_stats_dram_bytes_per_launch_C3")
-        return t.get("k_cluster_pass_dram_bytes_per_launch_" + workload,
-                     t.get("k_cluster_pass_dram_bytes_per_launch") if workload == "C2" else None)
-    return None
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -321,8 +320,7 @@ def run_reference_arm(args):
     if rank != 0:
         return
     shape = workload_shape(args.workload)
-    steps = max(1, min(args.steps, 3))
-    warm = 1 if args.warmup > 0 else 0
+    steps, warm = args.steps, args.warmup
     v, sec, desc = cpu_reference_run(steps, warm, shape["seed"])
     cores = min(os.cpu_count() or 1, 32)
     if v is None:
@@ -346,6 +344,14 @@ def run_reference_arm(args):
 # ---------------------------------------------------------------------------------------------
 # own arm
 # ---------------------------------------------------------------------------------------------
+def dump_outputs(out_dir, name, **arrays):
+    """what the last timed step handed back to its caller, as float64 .npy files (a few MB at most:
+    the Jones of C4 are 8 x 512 stations x 32 clusters doubles)"""
+    os.makedirs(out_dir, exist_ok=True)
+    for key, a in arrays.items():
+        np.save(os.path.join(out_dir, "%s_%s.npy" % (name, key)), np.asarray(a, dtype=np.float64))
+
+
 def n512_parity(api, variant="lm"):
     """reduced-interval problem at the station count of C4 (512 stations, 2 timeslots, 2 clusters)
     against the committed golden of the CPU restatement (tests/golden/n512): the parity evidence for
@@ -499,6 +505,8 @@ def run_workload(name, args, ctx, with_cpu=True):
         if world > 1:
             dist.barrier()
         clk = clocks.stop()
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, name, jones=pp, scalars=res)
         hstat = api.host_stats()
         ms_total = e0.elapsed_time(e1)
         launches = api.launch_count() - l0
@@ -614,7 +622,7 @@ def run_workload(name, args, ctx, with_cpu=True):
     n, ms, by = prof[names.index(dom)]
     achieved = (by / (ms * 1e-3)) / 1e9 if ms > 0 else 0.0
     roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": ncu_traffic(name), "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": peak_src,
                 "launches_in_timed_region": n, "avg_launch_us": 1e3 * ms / n if n else None,
                 "algorithmic_bytes_per_launch": by / n if n else None,
                 "profiled_ms_per_step": ms_profiled,
@@ -644,7 +652,7 @@ def run_workload(name, args, ctx, with_cpu=True):
                                                               pr.tilesz, R),
                    "solve": SOLVE_W, "sweeps_per_step": sweeps,
                    "units_per_step": "rows*clusters*(em_sweeps+lbfgs_grad_evals)",
-                   "l2": "inputs (%.0f MB coherencies per GPU) larger than the 126 MB L2, no flush needed"
+                   "l2": "inputs (%.0f MB coherencies per GPU) larger than the 50 MB L2, no flush needed"
                          % (coh_bytes / 1e6),
                    "coherencies": "generated on the device (dirac_b200_precalculate)" if devgen
                                   else "host array uploaded",
@@ -739,6 +747,8 @@ def run_consensus(args, ctx):
         if world > 1:
             dist.barrier()
         clk = clocks.stop()
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, "C5", jones=pp, history=hist)
         hstat = api.host_stats()
         launches = api.launch_count() - l0
         ms_total = e0.elapsed_time(e1)

@@ -1,5 +1,5 @@
 /*
- * dirac_b200 — Blackwell (sm_100a) implementation of the Dirac direction-dependent calibration hot
+ * dirac_b200 — Hopper (H100, sm_90a) implementation of the Dirac direction-dependent calibration hot
  * path.  C ABI only: plain pointers and sizes, host memory unless a name says otherwise.
  *
  * Two layers:

@@ -1,5 +1,5 @@
-"""TEST INFRASTRUCTURE ONLY: compares a product result with the oracle (compiled reference when
-oracle/_ref is present)."""
+"""TEST INFRASTRUCTURE ONLY: compares a product result with the compiled reference (its recorded
+answers, oracle/refreplay.py)."""
 import numpy as np
 
 import refdirac
@@ -8,9 +8,7 @@ import refdirac
 def check_sagefit(pr, barr, sky, pp_got, x_got, r0, r1, tol=1e-5, serial=False, **kw):
     """serial: against the reference build whose robust RTR / NSD solvers run their worker threads
     synchronously (the threaded build's nu update races, ref_shim_rtr_serial.c)"""
-    if not refdirac.available():
-        raise RuntimeError("oracle/_ref/libdirac_ref.so missing: run make -C oracle here first")
-    ref = refdirac.load_serial() if serial else refdirac.load()
+    ref = refdirac.recorded(serial)
     x = pr.x.copy()
     pp = pr.pp0.copy()
     args = dict(max_emiter=3, max_iter=5, max_lbfgs=10, lbfgs_m=7, solver_mode=1)

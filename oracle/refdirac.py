@@ -27,8 +27,8 @@ def available() -> bool:
 
 
 class RefDirac(DiracAPI):
-    def __init__(self, path: str = REF_PATH):
-        super().__init__(path)
+    def __init__(self, path: str = REF_PATH, lib=None):
+        super().__init__(path, lib)
         L = self.lib
         i, d, dp, vp = C.c_int, C.c_double, c_double_p, C.c_void_p
         L.ref_sizeof_me_data.restype = C.c_size_t
@@ -67,6 +67,10 @@ class RefDirac(DiracAPI):
         L.rtr_solve_nocuda_robust_admm.argtypes = [dp, dp, dp, dp, i, i, i, i, d, d, d, d, d, dp, vp]
         L.update_w_and_nu.restype = d
         L.update_w_and_nu.argtypes = [d, dp, dp, i, i, d, d]
+
+    def _callback(self, name):
+        fn = getattr(self.lib, name)
+        return C.cast(getattr(fn, "real", fn), C.c_void_p)
 
     # ---- me_data_t -------------------------------------------------------------------------
     def me_data(self, N, Nbase, tilesz, barr, sky: SkyModel, coh, clus=-1, tileoff=0, Nt=4,
@@ -120,8 +124,8 @@ class RefDirac(DiracAPI):
         pblk = np.ascontiguousarray(pblk, dtype=np.float64).copy()
         info = np.zeros(10)
         o = np.array(opts, dtype=np.float64)
-        f = C.cast(self.lib.ref_mylm_fit_single_pth0, C.c_void_p)
-        j = C.cast(self.lib.ref_mylm_jac_single_pth, C.c_void_p)
+        f = self._callback("ref_mylm_fit_single_pth0")
+        j = self._callback("ref_mylm_jac_single_pth")
         if os_:
             self.lib.oslevmar_der_single_nocuda(f, j, dptr(pblk), dptr(xd), len(pblk), len(xd),
                                                 itmax, dptr(o), dptr(info), linsolv, randomize, md)
@@ -135,8 +139,8 @@ class RefDirac(DiracAPI):
         """rlevmar_der_single_nocuda / osrlevmar_der_single_nocuda (robustlm.c:2008,2607)"""
         pblk = np.ascontiguousarray(pblk, dtype=np.float64).copy()
         info = np.zeros(10)
-        f = C.cast(self.lib.ref_mylm_fit_single_pth0, C.c_void_p)
-        j = C.cast(self.lib.ref_mylm_jac_single_pth, C.c_void_p)
+        f = self._callback("ref_mylm_fit_single_pth0")
+        j = self._callback("ref_mylm_jac_single_pth")
         if os_:
             self.lib.osrlevmar_der_single_nocuda(f, j, dptr(pblk), dptr(xd), len(pblk), len(xd),
                                                  itmax, None, dptr(info), linsolv, Nt, nulow,
@@ -180,6 +184,20 @@ class RefDirac(DiracAPI):
 
 _ref = None
 _ser = None
+_rec = {}
+
+
+def recorded(serial=False) -> RefDirac:
+    """the reference as tests and smoke() see it: its stored answers (refreplay, tests/golden/ref),
+    or, with DIRAC_REF_RECORD set, the compiled library with every answer recorded"""
+    if serial not in _rec:
+        import refreplay
+        path = SERIAL_PATH if serial else REF_PATH
+        if refreplay.RECORD_DIR:
+            _rec[serial] = RefDirac(path, refreplay.RecordLib(C.CDLL(path, mode=C.RTLD_GLOBAL)))
+        else:
+            _rec[serial] = RefDirac(path, refreplay.ReplayLib(path))
+    return _rec[serial]
 
 
 def load_serial() -> RefDirac:

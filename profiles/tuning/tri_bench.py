@@ -1,4 +1,4 @@
-import sys; sys.path.insert(0,'/root/repo')
+import sys, os; sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import ctypes as C, numpy as np
 from sagecal_b200 import lib as blib
 L = blib.load().lib

@@ -1,4 +1,4 @@
-// Internal declarations shared by the sm_100a kernels and the host-side solver code.
+// Internal declarations shared by the sm_90a kernels and the host-side solver code.
 // Nothing here is part of the public C-ABI (see include/dirac_b200.h).
 #pragma once
 #include <cuda_runtime.h>

@@ -955,7 +955,7 @@ void db_launch_chol_solve(const double *A, int n, double mu, const double *b, do
 
 // Batched factorisation: nb matrices A[b] (n x n, stride n*n), A[b] + mu[b] I = L L^T, one thread-block
 // cluster each, all concurrent (the batch of first systems of a SAGE sweep: 64 clusters of 16 CTAs on
-// 148 SMs run nine at a time).  Factor b lands at ws + b*ws_stride with ld = 32*ceil(n/32);
+// 132 SMs run eight at a time).  Factor b lands at ws + b*ws_stride with ld = 32*ceil(n/32);
 // info[2b] as dpotrf.  Replaces cusolverDnDpotrfBatched on this path.
 void db_launch_chol_factor_batched(const double *A, int n, const double *mu, double *ws,
                                    long long ws_stride, int *info, int nb, cudaStream_t st) {
@@ -965,8 +965,8 @@ void db_launch_chol_factor_batched(const double *A, int n, const double *mu, dou
   p.A = A; p.b = nullptr; p.x = nullptr; p.ws = ws; p.info = info; p.mu = 0.0; p.n = n;
   p.nblk = (n + 31) / 32;
   p.factor_only = 1; p.mu_ptr = mu; p.ws_stride = ws_stride;
-  // Throughput, not latency, counts for the batch: small clusters (4 CTAs) keep 37 matrices in flight
-  // on 148 SMs and spend less of their time in cluster barriers than the 16-CTA shape of a lone solve
+  // Throughput, not latency, counts for the batch: small clusters (4 CTAs) keep 33 matrices in flight
+  // on 132 SMs and spend less of their time in cluster barriers than the 16-CTA shape of a lone solve
   static int bcl = -1;
   if (bcl < 0) {
     const char *e = getenv("DIRAC_B200_BATCH_CL");

@@ -1,4 +1,4 @@
-// Streaming sm_100a kernels of the calibration E-step: every kernel makes one pass over planar
+// Streaming sm_90a kernels of the calibration E-step: every kernel makes one pass over planar
 // coherencies / visibilities in HBM with 128-bit coalesced loads (a warp = one station p against
 // 32 consecutive stations q, 512 contiguous bytes per polarisation product per timeslot).
 //

@@ -23,7 +23,7 @@ template <int MODE, int TB, int NST, int WARPS, bool PF>
 __global__ void __launch_bounds__(WARPS * 32)
 k_stream_all(StreamAllArgs a) {
   // One CTA = one item (32 consecutive baselines x TB timeslots); its WARPS warps split the clusters
-  // (k = w, w+WARPS, ...) so that the grid has many small CTAs (little tail on 148 SMs) and every
+  // (k = w, w+WARPS, ...) so that the grid has many small CTAs (little tail on 132 SMs) and every
   // warp runs its own producer/consumer ring.  The partial models are combined through shared
   // memory in warp order (deterministic), warp 0 finishes the rows.
   extern __shared__ __align__(128) unsigned char smem_raw[];

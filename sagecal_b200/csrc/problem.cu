@@ -88,10 +88,10 @@ extern "C" int dirac_b200_set_option(const char *name, int value) {
 int db_sm_count() {
   static int n[64];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (!n[dev]) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     n[dev] = v;
   }
   return n[dev];
@@ -114,9 +114,9 @@ static void require_gpu() {
 // cost milliseconds to hundreds of milliseconds (32 GB of coherencies at 512 stations: 50-350 ms
 // measured) and serialise the device, so freed blocks are kept and handed out again when a request
 // of exactly the same size comes back (the driver calls with the same shapes tile after tile).
-// Bounded: the cache holds at most 40 % of the device's memory (a 512-station shard with its solver
-// workspaces is 55 GB; $DIRAC_B200_CACHE_GB overrides, 0 disables); a failed cudaMalloc gives the
-// whole cache back and retries once;
+// Bounded: the cache holds at most 75 % of the device's memory, so that a 512-station shard with its
+// solver workspaces (55 GB) stays cached on an 80 GB H100 ($DIRAC_B200_CACHE_GB overrides, 0
+// disables); a failed cudaMalloc gives the whole cache back and retries once;
 // dirac_b200_release_cache() empties it on request.
 #include <map>
 #include <unordered_map>
@@ -131,7 +131,7 @@ static size_t cache_cap() {
       cap = (size_t)(atof(e) * 1073741824.0);
     } else {
       size_t fr = 0, tot = 0;
-      cap = (cudaMemGetInfo(&fr, &tot) == cudaSuccess) ? tot / 5 * 2 : ((size_t)6 << 30);
+      cap = (cudaMemGetInfo(&fr, &tot) == cudaSuccess) ? tot / 4 * 3 : ((size_t)6 << 30);
     }
   }
   return cap;

@@ -227,9 +227,9 @@ def barr_to_numpy(barr, n):
 class DiracAPI:
     """Binds the hot-path entry points of a Dirac-ABI shared library."""
 
-    def __init__(self, path: str):
+    def __init__(self, path: str, lib=None):
         self.path = path
-        self.lib = C.CDLL(path, mode=C.RTLD_GLOBAL)
+        self.lib = lib if lib is not None else C.CDLL(path, mode=C.RTLD_GLOBAL)
         L = self.lib
         bp = C.POINTER(baseline_t)
         cp = C.POINTER(clus_source_t)

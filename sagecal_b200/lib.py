@@ -1,4 +1,4 @@
-"""Loader for the product library `libdirac_b200.so` (hand-written sm_100a kernels behind the
+"""Loader for the product library `libdirac_b200.so` (hand-written sm_90a kernels behind the
 Dirac C API).  There is no CPU fallback: a missing library or a missing GPU is an error."""
 from __future__ import annotations
 

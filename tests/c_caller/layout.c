@@ -1,6 +1,7 @@
 /* TEST ONLY.  Prints size, field offsets and enumerated constants of every struct / macro the C ABI
- * shares with the reference; compiled twice (reference headers with -DUSE_REF, include/dirac_b200.h
- * without) by tests/test_c_caller.py::test_struct_layouts_equal_the_reference_headers. */
+ * shares with the reference; compiled against include/dirac_b200.h by
+ * tests/test_c_caller.py::test_struct_layouts_equal_the_reference_headers, and against the reference
+ * headers (-DUSE_REF) by tests/golden/make_golden_headers.py, whose output the test compares with. */
 #include <stddef.h>
 #include <stdio.h>
 #ifdef USE_REF

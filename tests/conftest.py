@@ -9,16 +9,15 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
 def ref():
-    """compiled reference CPU path (oracle/_ref), test infrastructure only"""
+    """the compiled reference CPU path (oracle/_ref), test infrastructure only: its recorded answers
+    (tests/golden/ref), or the live library recording them when DIRAC_REF_RECORD is set"""
     import refdirac
-    if not refdirac.available():
-        pytest.skip("oracle/_ref/libdirac_ref.so not built (make -C oracle)")
-    return refdirac.load()
+    return refdirac.recorded()
 
 
 @pytest.fixture(scope="session")
@@ -26,10 +25,7 @@ def refser():
     """the compiled reference with the worker threads of its robust RTR / NSD solvers run
     synchronously (oracle/ref_shim_rtr_serial.c): deterministic pin of solver_mode 5 and 6"""
     import refdirac
-    import os
-    if not os.path.exists(refdirac.SERIAL_PATH):
-        pytest.skip("oracle/_ref/libdirac_ref_serial.so not built (make -C oracle)")
-    return refdirac.load_serial()
+    return refdirac.recorded(serial=True)
 
 
 @pytest.fixture(scope="session")

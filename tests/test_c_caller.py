@@ -33,14 +33,25 @@ def test_c_host_runs_the_solver(tmp_path):
     assert out.returncode == 0 and "C_CALLER OK" in out.stdout, (out.returncode, out.stdout, out.stderr)
 
 
+# every name link_order.c looks up: the hot-path entry points and three reference-only helpers
+LINK_ORDER_SYMBOLS = ["sagefit_visibilities", "sagefit_visibilities_dual_pt_flt", "bfgsfit_visibilities",
+                      "bfgsfit_visibilities_gpu", "precalculate_coherencies",
+                      "precalculate_coherencies_withbeam_gpu", "predict_visibilities_multifreq",
+                      "calculate_residuals_multifreq", "sagefit_visibilities_admm",
+                      "bfgsfit_minibatch_visibilities", "lbfgs_persist_init", "generate_baselines",
+                      "preset_flags_and_data", "whiten_data", "my_dscal", "my_dnrm2", "update_w_and_nu"]
+
+
 def test_link_order_puts_the_hot_path_on_this_library(tmp_path):
-    """INTEGRATION.md section 2 on a CPU box: `-ldirac_b200` in front of the reference's library
-    (oracle/_ref, the reference CPU path compiled from its own sources) takes over the hot-path
-    symbols and leaves the rest with the reference."""
-    refdir = os.path.join(ROOT, "oracle", "_ref")
-    if not os.path.exists(os.path.join(refdir, "libdirac_ref.so")):
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
-    exe = os.path.join(str(tmp_path), "link_order")
+    """INTEGRATION.md section 2 on a CPU box: `-ldirac_b200` in front of the reference's library takes
+    over the hot-path symbols and leaves the rest with the reference.  The reference's library is
+    stood in for by one that, like it, defines every name link_order.c looks up."""
+    refdir = str(tmp_path)
+    stub = os.path.join(refdir, "dirac_ref_standin.c")
+    with open(stub, "w") as f:
+        f.write("".join("void %s(void) {}\n" % s for s in LINK_ORDER_SYMBOLS))
+    subprocess.check_call(["gcc", "-shared", "-fPIC", "-o", os.path.join(refdir, "libdirac_ref.so"), stub])
+    exe = os.path.join(refdir, "link_order")
     libdir = os.path.join(ROOT, "sagecal_b200")
     cmd = ["gcc", "-O1", "-Wall", "-o", exe, os.path.join(ROOT, "tests", "c_caller", "link_order.c"),
            "-I", os.path.join(ROOT, "include"), "-L", libdir, "-ldirac_b200", "-L", refdir,
@@ -50,6 +61,7 @@ def test_link_order_puts_the_hot_path_on_this_library(tmp_path):
     out = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, (out.stdout, out.stderr)
     got = dict(line.split() for line in out.stdout.strip().splitlines())
+    assert sorted(got) == sorted(LINK_ORDER_SYMBOLS), got
     ours = [s for s, lib in got.items() if lib == "libdirac_b200.so"]
     theirs = [s for s, lib in got.items() if lib == "libdirac_ref.so"]
     assert sorted(theirs) == ["my_dnrm2", "my_dscal", "update_w_and_nu"], got
@@ -59,15 +71,12 @@ def test_link_order_puts_the_hot_path_on_this_library(tmp_path):
 def test_struct_layouts_equal_the_reference_headers(tmp_path):
     """baseline_t, clus_source_t, exinfo_*, elementcoeff, the prefix of persistent_data_t and the
     STYPE_ / DOBEAM_ / STAT_ / SM_ constants: same sizes, offsets and values as a caller compiled
-    against the reference's Dirac.h / Dirac_radio.h sees (74 lines compared)."""
-    refinc = "/root/reference/src/lib"
-    if not os.path.isdir(refinc):
-        pytest.skip("reference headers not present on this box")
-    src = os.path.join(ROOT, "tests", "c_caller", "layout.c")
-    outs = []
-    for name, flags in (("ref", ["-DUSE_REF", "-I", refinc + "/Dirac", "-I", refinc + "/Radio"]),
-                        ("ours", ["-I", os.path.join(ROOT, "include")])):
-        exe = os.path.join(str(tmp_path), name)
-        subprocess.check_call(["gcc", "-w", "-o", exe, src] + flags)
-        outs.append(subprocess.run([exe], capture_output=True, text=True, timeout=60).stdout)
-    assert outs[0] == outs[1] and len(outs[0].splitlines()) > 70
+    against the reference's Dirac.h / Dirac_radio.h sees (74 lines compared; the reference's side is
+    stored, tests/golden/make_golden_headers.py)."""
+    exe = os.path.join(str(tmp_path), "ours")
+    subprocess.check_call(["gcc", "-w", "-o", exe, os.path.join(ROOT, "tests", "c_caller", "layout.c"),
+                           "-I", os.path.join(ROOT, "include")])
+    ours = subprocess.run([exe], capture_output=True, text=True, timeout=60).stdout
+    with open(os.path.join(ROOT, "tests", "golden", "ref_layout.txt")) as f:
+        ref = f.read()
+    assert ours == ref and len(ref.splitlines()) > 70

@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def test_sharded_matches_single_gpu():
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
            "--master-addr", "127.0.0.1", "--master-port", "29617",
            os.path.join(ROOT, "tests", "mgpu_check.py")]
@@ -24,7 +24,7 @@ def test_sharded_matches_single_gpu():
 def test_consensus_over_subbands():
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
            "--master-addr", "127.0.0.1", "--master-port", "29618",
            os.path.join(ROOT, "tests", "consensus_check.py")]

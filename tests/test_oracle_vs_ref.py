@@ -1,5 +1,6 @@
 """CPU: pins the restated oracle (oracle/dirac_oracle.c) against the compiled reference
-(oracle/_ref, built from /root/reference by oracle/Makefile).  Runs without a GPU."""
+(oracle/_ref, built from the reference sources by oracle/Makefile; its answers are replayed from
+tests/golden/ref where it is not built).  Runs without a GPU."""
 import numpy as np
 import pytest
 

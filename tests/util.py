@@ -29,6 +29,12 @@ def perturbed_jones(pr, seed=3, amp=0.1):
 
 
 def relerr(a, b):
+    """max |a - b| / max |b|.  b is the reference: where it is a stored sample of a large reference
+    answer (oracle/refreplay.py leaves the elements outside the sample NaN) only the sample counts"""
     a = np.asarray(a)
     b = np.asarray(b)
+    keep = ~np.isnan(b)
+    if not keep.all():
+        assert keep.any(), "no reference value to compare with"
+        a, b = np.broadcast_to(a, b.shape)[keep], b[keep]
     return float(np.max(np.abs(a - b)) / (np.max(np.abs(b)) + 1e-300))
