@@ -499,9 +499,13 @@ void dirac_b200_host_stats(unsigned long long *syncs, double *wait_seconds, int 
  * (replaces dpotrf + dpotrs of clmfit.c:373-395).  Host buffers.  *info as dpotrf (0, or the index
  * of the first non-positive pivot).  Returns 0, or -1 if the device grants no 8/16-CTA cluster.
  * dirac_b200_tri_solve: L L^T x = b for an existing factor L (column-major lower, ld = n), i.e.
- * dpotrs; reps > 0 additionally times `reps` back-to-back solves (us per solve in *us). */
+ * dpotrs; reps > 0 additionally times `reps` back-to-back solves (us per solve in *us).
+ * dirac_b200_tri_solve_ld: the same for a factor with leading dimension ld >= n (the batched
+ * factorisation of the LM leaves its factors at ld = 32*ceil(n/32)). */
 int dirac_b200_spd_solve(int n, const double *A, const double *b, double mu, double *x, int *info);
 int dirac_b200_tri_solve(int n, const double *L, const double *b, double *x, int reps, double *us);
+int dirac_b200_tri_solve_ld(int n, const double *L, int ld, const double *b, double *x, int reps,
+                            double *us);
 /* the same for systems beyond the cluster kernels (n > 512, a multiple of 64, e.g. 4096 at 512
  * stations): blocked dataflow substitutions over n/64 co-resident CTAs (replaces cusolverDnDpotrs
  * behind cuSOLVER's dpotrf).  Returns -1 when the size is not handled. */

@@ -418,4 +418,7 @@ void db_launch_bigtri_solve(const double *L, int ld, int n, const double *b, dou
 int db_stream_all_nblocks(int Nbase, int tilesz);
 void db_launch_predict_tma(const StreamAllArgs *a, cudaStream_t st);
 void db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st);
+// (TB, NST, WARPS) of the last k_stream_all<1> launch since the reset (-1 each: none)
+void db_line_setup_shape_reset();
+void db_line_setup_shape(int *shape);
 }

@@ -1031,22 +1031,24 @@ void db_launch_tri_solve_ld(const double *L, int ld, int n, const double *b, dou
   DB_CHECK(cudaLaunchKernelEx(&cfg, k_tri_solve, p));
 }
 
-// test hook: x = (L L^T)^-1 b from host buffers; returns -1 when the cluster solver is unavailable
-int dirac_b200_tri_solve(int n, const double *L, const double *b, double *x, int reps, double *us) {
-  if (!db_tri_available(n)) return -1;
+// test hook: x = (L L^T)^-1 b from host buffers (L column-major lower with leading dimension
+// ld >= n); returns -1 when the cluster solver is unavailable
+int dirac_b200_tri_solve_ld(int n, const double *L, int ld, const double *b, double *x, int reps,
+                            double *us) {
+  if (!db_tri_available(n) || ld < n) return -1;
   double *dL, *db, *dx;
-  DB_CHECK(cudaMalloc(&dL, sizeof(double) * n * n));
+  DB_CHECK(cudaMalloc(&dL, sizeof(double) * ld * n));
   DB_CHECK(cudaMalloc(&db, sizeof(double) * n));
   DB_CHECK(cudaMalloc(&dx, sizeof(double) * n));
-  DB_CHECK(cudaMemcpy(dL, L, sizeof(double) * n * n, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(dL, L, sizeof(double) * ld * n, cudaMemcpyHostToDevice));
   DB_CHECK(cudaMemcpy(db, b, sizeof(double) * n, cudaMemcpyHostToDevice));
-  db_launch_tri_solve(dL, n, db, dx, 0);
+  db_launch_tri_solve_ld(dL, ld, n, db, dx, 0);
   DB_CHECK(cudaMemcpy(x, dx, sizeof(double) * n, cudaMemcpyDeviceToHost));
   if (reps > 0 && us) {
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0); cudaEventCreate(&e1);
     cudaEventRecord(e0, 0);
-    for (int i = 0; i < reps; i++) db_launch_tri_solve(dL, n, db, dx, 0);
+    for (int i = 0; i < reps; i++) db_launch_tri_solve_ld(dL, ld, n, db, dx, 0);
     cudaEventRecord(e1, 0);
     DB_CHECK(cudaEventSynchronize(e1));
     float ms = 0.f;
@@ -1056,6 +1058,38 @@ int dirac_b200_tri_solve(int n, const double *L, const double *b, double *x, int
   }
   cudaFree(dL); cudaFree(db); cudaFree(dx);
   return 0;
+}
+
+// test hook: the batched factorisation of the LM's per-sweep batch from host buffers.  A: nb
+// column-major n x n matrices back to back (only the lower triangles are read), mu: nb dampings.
+// L: nb factors of A[b] + mu[b] I, each column-major ld x ld with ld = 32*ceil(n/32) as the solver
+// leaves them (lower triangle of the leading n x n block; the rest is not part of the factor).
+// info: 2*nb ints, info[2b] as dpotrf.  Returns -1 when the batch does not run on the cluster kernel
+// (the LM then factorises with cuSOLVER).
+int dirac_b200_chol_factor_batched(int n, int nb, const double *A, const double *mu, double *L,
+                                   int *info) {
+  if (!db_tri_available(n) || nb < 1) return -1;
+  const size_t ld = (size_t)32 * ((n + 31) / 32), stride = db_chol_ws_doubles(n);
+  double *dA, *dmu, *dws;
+  int *dinfo;
+  DB_CHECK(cudaMalloc(&dA, sizeof(double) * n * n * nb));
+  DB_CHECK(cudaMalloc(&dmu, sizeof(double) * nb));
+  DB_CHECK(cudaMalloc(&dws, sizeof(double) * stride * nb));
+  DB_CHECK(cudaMalloc(&dinfo, sizeof(int) * 2 * nb));
+  DB_CHECK(cudaMemset(dws, 0, sizeof(double) * stride * nb));
+  DB_CHECK(cudaMemcpy(dA, A, sizeof(double) * n * n * nb, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(dmu, mu, sizeof(double) * nb, cudaMemcpyHostToDevice));
+  db_launch_chol_factor_batched(dA, n, dmu, dws, (long long)stride, dinfo, nb, 0);
+  for (int b = 0; b < nb; b++)
+    DB_CHECK(cudaMemcpy(L + ld * ld * b, dws + stride * b, sizeof(double) * ld * ld,
+                        cudaMemcpyDeviceToHost));
+  DB_CHECK(cudaMemcpy(info, dinfo, sizeof(int) * 2 * nb, cudaMemcpyDeviceToHost));
+  cudaFree(dA); cudaFree(dmu); cudaFree(dws); cudaFree(dinfo);
+  return 0;
+}
+
+int dirac_b200_tri_solve(int n, const double *L, const double *b, double *x, int reps, double *us) {
+  return dirac_b200_tri_solve_ld(n, L, n, b, x, reps, us);
 }
 
 // test hook: out[i] = fast_rsqrt(in[i]) as the pivots see it

@@ -246,8 +246,15 @@ k_stream_all(StreamAllArgs a) {
 #define SA_TB0 2  // predict
 #define SA_TB1 2  // line setup
 
+static int g_line_shape[3] = {-1, -1, -1};  // shape of the last line-model launch (tests)
+
 template <int MODE, int TB, int NST, int WARPS, bool PF>
 static void launch_cfg(const StreamAllArgs *a, cudaStream_t st) {
+  if (MODE == 1) {
+    g_line_shape[0] = TB;
+    g_line_shape[1] = NST;
+    g_line_shape[2] = WARPS;
+  }
   const int nbg = (a->Nbase + 31) / 32, ntb = (a->tilesz + TB - 1) / TB;
   const unsigned grid = (unsigned)((long long)nbg * ntb);
   constexpr int NACC = (MODE == 0) ? 1 : 3;
@@ -338,5 +345,9 @@ void db_launch_predict_tma(const StreamAllArgs *a, cudaStream_t st) {
 }
 void db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st) {
   launch_stream_all<1, SA_TB1>(a, st);
+}
+void db_line_setup_shape_reset() { g_line_shape[0] = g_line_shape[1] = g_line_shape[2] = -1; }
+void db_line_setup_shape(int *shape) {
+  for (int i = 0; i < 3; i++) shape[i] = g_line_shape[i];
 }
 }

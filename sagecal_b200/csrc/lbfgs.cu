@@ -376,6 +376,45 @@ void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, in
   db_free(ws);
 }
 
+// test hook: the line model of the resident problem along pk from xk (host vectors of npar doubles),
+// exactly as one LBFGS iteration of a single-GPU solve sets it up.  Out (host):
+//   E       3 x 8R doubles, E0 | E1 | E2 in API layout (e(a) = E0 - a E1 - a^2 E2)
+//   poly    the 5 coefficients of the Gaussian cost along the line (k_line_poly)
+//   costs   [2 * nalpha]: k_line_eval at alphas[i], Gaussian (2i) and Student's-t with nu (2i + 1)
+//   res     8R doubles: k_line_residual at alpha_res, API layout
+//   shape   (TB, NST, WARPS) of the k_stream_all<1> launch that ran, or (0, 0, 0) for the
+//           register-staged k_line_setup (DIRAC_B200_NO_TMA)
+extern "C" void dirac_b200_line_model(dirac_b200_problem *pr, const double *xk, const double *pk,
+                                      int nalpha, const double *alphas, double nu,
+                                      double alpha_res, double *E, double *poly, double *costs,
+                                      double *res, int *shape) {
+  DevProblem &d = pr->d;
+  LbfgsCtx c;
+  c.pr = pr; c.robust = 0; c.nu = nu; c.m = (int)d.npar; c.ncost = c.ngrad = 0;
+  double *dx = (double *)db_malloc(sizeof(double) * 2 * d.npar);
+  double *dp = dx + d.npar;
+  DB_CHECK(cudaMemcpyAsync(dx, xk, sizeof(double) * d.npar, cudaMemcpyHostToDevice, d.stream));
+  DB_CHECK(cudaMemcpyAsync(dp, pk, sizeof(double) * d.npar, cudaMemcpyHostToDevice, d.stream));
+  db_line_setup_shape_reset();
+  line_setup(&c, dx, dp);
+  if (db_use_tma()) db_line_setup_shape(shape);
+  else shape[0] = shape[1] = shape[2] = 0;
+  for (int j = 0; j < 5; j++) poly[j] = c.poly[j];
+  for (int i = 0; i < nalpha; i++)
+    for (int mode = 1; mode <= 2; mode++) {
+      db_launch_line_eval(pr->E0, pr->E1, pr->E2, 4 * d.R, alphas[i], mode,
+                          mode == 2 ? 1.0 / nu : 0.0, pr->partials, d.scal, d.counters, d.stream);
+      costs[2 * i + mode - 1] = db_read_scalar(pr, 0);
+    }
+  db_download_vis(pr, pr->E0, E);
+  db_download_vis(pr, pr->E1, E + 8 * d.R);
+  db_download_vis(pr, pr->E2, E + 16 * d.R);
+  db_launch_line_residual(pr->E0, pr->E1, pr->E2, pr->res, 4 * d.R, alpha_res, d.stream);
+  db_download_vis(pr, pr->res, res);
+  DB_CHECK(cudaGetLastError());
+  db_free(dx);
+}
+
 // micro-benchmark of the line-model setup on the resident problem (direction = current Jones):
 // average device time (us) of `reps` back-to-back launches
 extern "C" double dirac_b200_bench_line_setup(dirac_b200_problem *pr, int reps) {

@@ -22,7 +22,7 @@ EXPORTED = [
     "dirac_b200_grad", "dirac_b200_normal_eq", "dirac_b200_launch_count", "dirac_b200_sagefit",
     "dirac_b200_set_stream", "dirac_b200_profile_enable", "dirac_b200_profile_read",
     "dirac_b200_kernel_count", "dirac_b200_normal_eq_weighted", "dirac_b200_create_shard",
-    "dirac_b200_set_comm", "dirac_b200_spd_solve", "dirac_b200_tri_solve",
+    "dirac_b200_set_comm", "dirac_b200_spd_solve", "dirac_b200_tri_solve", "dirac_b200_tri_solve_ld",
     "dirac_b200_set_option", "dirac_b200_nccl_unique_id", "dirac_b200_nccl_init",
     "dirac_b200_nccl_finalize", "dirac_b200_nccl_ready", "dirac_b200_comm_stats",
     "dirac_b200_noise_decisions", "dirac_b200_host_stats", "dirac_b200_consensus_basis",
@@ -182,6 +182,29 @@ class DeviceProblem:
                                              solver_mode, nulow, nuhigh, randomize, C.byref(nu),
                                              C.byref(r0), C.byref(r1))
         return rv, nu.value, r0.value, r1.value
+
+    def line_model(self, xk, pk, alphas, nu, alpha_res):
+        """the LBFGS line model along pk from xk as one iteration sets it up (dirac_b200_line_model).
+        returns dict(E0, E1, E2 [API layout], poly [5], cost_gauss, cost_robust [per alpha],
+        res [line residual at alpha_res], shape (TB, NST, WARPS) of the k_stream_all<1> launch or
+        (0, 0, 0) for the register-staged k_line_setup)"""
+        L = self.api.lib
+        L.dirac_b200_line_model.restype = None
+        L.dirac_b200_line_model.argtypes = [C.c_void_p, c_double_p, c_double_p, C.c_int, c_double_p,
+                                            C.c_double, C.c_double, c_double_p, c_double_p, c_double_p,
+                                            c_double_p, C.POINTER(C.c_int)]
+        xk = np.ascontiguousarray(xk, dtype=np.float64)
+        pk = np.ascontiguousarray(pk, dtype=np.float64)
+        alphas = np.ascontiguousarray(alphas, dtype=np.float64)
+        E = np.zeros(3 * self.n)
+        poly = np.zeros(5)
+        costs = np.zeros(2 * len(alphas))
+        res = np.zeros(self.n)
+        shape = (C.c_int * 3)()
+        L.dirac_b200_line_model(self.h, dptr(xk), dptr(pk), len(alphas), dptr(alphas), nu, alpha_res,
+                                dptr(E), dptr(poly), dptr(costs), dptr(res), shape)
+        return dict(E0=E[:self.n], E1=E[self.n:2 * self.n], E2=E[2 * self.n:], poly=poly,
+                    cost_gauss=costs[0::2], cost_robust=costs[1::2], res=res, shape=tuple(shape))
 
     def normal_eq(self, clus, chunk, pblk, xd):
         n8 = 8 * self.N

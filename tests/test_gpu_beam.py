@@ -155,3 +155,38 @@ def test_coherencies_multifreq_withbeam(api, ref, mode, tile):
                                                      b.fresh_barr(), sky, f, pr.fdelta, one,
                                                      uvmin=30.0, uvmax=1e5)
         assert relerr(got[c * n:(c + 1) * n], want) < 1e-10, (c, relerr(got[c * n:(c + 1) * n], want))
+
+
+def test_segmented_cluster_split_withbeam(api):
+    """station beams on (array factor of a tile beam-former): a 200-source cluster, staged by the
+    coherency kernel in three segments, has the coherencies of the same sources as three clusters of
+    at most 96 summed, and subtracts the same residual as they do with equal Jones (3 channels)"""
+    from util import big_cluster_sky, split_cluster
+    freqs = np.array([146e6, 152e6, 158e6])
+    b, _, beam = beam_problem(None, "array", True, seed=43, freqs=freqs)
+    pr = b.pr
+    rng = np.random.default_rng(43)
+    cls = big_cluster_sky(seed=11, sizes=(1, 200))
+    for cl in cls:
+        K = len(cl["ll"])
+        cl["ra"] = 1.2 + np.deg2rad(rng.uniform(-4, 4, K))
+        cl["dec"] = np.deg2rad(58.0) + np.deg2rad(rng.uniform(-4, 4, K))
+    split = [cls[0]] + split_cluster(cls[1], (96, 96, 8))
+    cw = api.precalculate_coherencies_withbeam(pr.u, pr.v, pr.w, pr.N, pr.Nbase1, b.fresh_barr(),
+                                               SkyModel(cls, pr.N), pr.freq0, pr.fdelta, beam)
+    cs = api.precalculate_coherencies_withbeam(pr.u, pr.v, pr.w, pr.N, pr.Nbase1, b.fresh_barr(),
+                                               SkyModel(split, pr.N), pr.freq0, pr.fdelta, beam)
+    cw, cs = cw.reshape(pr.Nbase1, 2, 4), cs.reshape(pr.Nbase1, 4, 4)
+    assert np.array_equal(cs[:, 0], cw[:, 0])
+    assert relerr(cs[:, 1:].sum(axis=1), cw[:, 1]) < 1e-12
+    J = [pr.pp0[:8 * pr.N] + 0.1 * rng.normal(0, 1, 8 * pr.N) for _ in range(2)]
+    x0 = rng.normal(0, 1, 8 * pr.Nbase1 * len(freqs))
+    out = []
+    for sky_cls, p in ((cls, J), (split, [J[0], J[1], J[1], J[1]])):
+        x = x0.copy()
+        api.calculate_residuals_multifreq_withbeam(pr.u, pr.v, pr.w, np.concatenate(p), x, pr.N,
+                                                   pr.Nbase, pr.tilesz, b.barr,
+                                                   SkyModel(sky_cls, pr.N), freqs, pr.fdelta * 3, beam)
+        out.append(x)
+    assert relerr(out[1] - x0, out[0] - x0) < 1e-12
+    assert relerr(out[0], x0) > 1e-3

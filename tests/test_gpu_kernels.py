@@ -251,3 +251,144 @@ def test_calculate_residuals_multifreq(api, ref, ccid, nchunk, phase_only):
     # manifold_average.c:399-610, restated on the host with its own 3x3 eigen-solver)
     assert relerr(xb, xa) < (1e-9 if phase_only else 1e-11)
     assert relerr(xa, x0) > 1e-3   # something was subtracted
+
+
+# ---- sky models whose clusters span several staging segments ------------------------------------
+# k_sky_predict stages a cluster's sources COH_SEG_MAX = 96 at a time and carries the cluster's sum
+# from segment to segment until the one that closes it.  Clusters of 1, 95, 96, 97, 192 and 200
+# sources and an empty one make 11 segments: with several channels the double-buffer parity of a
+# segment flips from one channel to the next.
+
+def _segment_sky():
+    from sagecal_b200.dirac_api import SkyModel
+    from util import big_cluster_sky
+    b = small_problem(N=9, M=2, tilesz=5, seed=91)
+    clusters = big_cluster_sky()
+    return b, clusters, SkyModel(clusters, b.pr.N)
+
+
+def test_coherencies_segmented_clusters(api):
+    import orcdirac
+    b, clusters, sky = _segment_sky()
+    pr = b.pr
+    want = orcdirac.OracleSky(clusters).coherencies(pr.u, pr.v, pr.w, pr.freq0, pr.fdelta)
+    got = api.precalculate_coherencies(pr.u, pr.v, pr.w, pr.N, pr.Nbase1, b.fresh_barr(), sky,
+                                       pr.freq0, pr.fdelta)
+    got, want = got.reshape(pr.Nbase1, -1, 4), want.reshape(pr.Nbase1, -1, 4)
+    for k in range(len(clusters) - 1):
+        assert relerr(got[:, k], want[:, k]) < 1e-11, k
+    # the empty cluster: zero coherencies
+    assert not got[:, -1].any()
+
+
+@pytest.mark.parametrize("nchan", [1, 2, 3])
+def test_predict_multifreq_segmented_clusters(api, nchan):
+    import orcdirac
+    b, clusters, sky = _segment_sky()
+    pr = b.pr
+    freqs = np.array([146e6, 152e6, 158e6])[:nchan]
+    xa = orcdirac.OracleSky(clusters).predict_multifreq(pr.u, pr.v, pr.w, freqs, pr.fdelta * nchan, 1,
+                                                        np.zeros(8 * pr.Nbase1 * nchan))
+    xb = np.full(8 * pr.Nbase1 * nchan, np.nan)
+    api.predict_visibilities_multifreq(pr.u, pr.v, pr.w, xb, pr.N, pr.Nbase, pr.tilesz, b.barr, sky,
+                                       freqs, pr.fdelta * nchan, add_to_data=1)
+    assert relerr(xb, xa) < 1e-11
+
+
+def test_residual_split_cluster_identity(api):
+    """a 200-source cluster subtracts what the same sources do as three clusters of at most 96
+    with equal Jones (calculate_residuals_multifreq, 3 channels)"""
+    from sagecal_b200.dirac_api import SkyModel
+    from util import big_cluster_sky, split_cluster
+    b, clusters, _ = _segment_sky()
+    pr = b.pr
+    whole = [clusters[0], clusters[5]]
+    split = [clusters[0]] + split_cluster(clusters[5], (96, 96, 8))
+    rng = np.random.default_rng(6)
+    J = [pr.pp0[:8 * pr.N] + 0.1 * rng.normal(0, 1, 8 * pr.N) for _ in range(2)]
+    freqs = np.array([146e6, 152e6, 158e6])
+    x0 = rng.normal(0, 1, 8 * pr.Nbase1 * len(freqs))
+    out = []
+    for cls, p in ((whole, J), (split, [J[0], J[1], J[1], J[1]])):
+        x = x0.copy()
+        assert api.calculate_residuals_multifreq(pr.u, pr.v, pr.w, np.concatenate(p), x, pr.N,
+                                                 pr.Nbase, pr.tilesz, b.fresh_barr(),
+                                                 SkyModel(cls, pr.N), freqs, pr.fdelta * 3) == 0
+        out.append(x)
+    assert relerr(out[1] - x0, out[0] - x0) < 1e-12
+    assert relerr(out[0], x0) > 1e-3
+
+
+# ---- station-count edges of the per-row passes ----------------------------------------------------
+# 2 stations: one baseline; 3: a single lane of a 32-baseline group; 9: 36 baselines, a ragged
+# group; 33, 65: partial 8 x 32 tiles; 100: 4950 baselines (several 256-baseline groups of the
+# linear cluster pass) and 8N = 800 normal equations.  Against the restatement (oracle/liboracle.so).
+
+EDGE_N = [2, 3, 9, 33, 65, 100]
+
+
+@pytest.fixture(params=EDGE_N, ids=lambda n: "N%d" % n)
+def edge(request):
+    import orcdirac
+    N = request.param
+    b = small_problem(N=N, M=3, tilesz=6 if N < 65 else 3, seed=200 + N, kmean=1.0,
+                      nchunk=[1, 2, 1], flag_frac=0.05 if N < 4 else 0.01,
+                      uvcut_frac=0.0 if N < 4 else 0.005)
+    return b, orcdirac.Oracle(b.pr)
+
+
+def test_predict_station_edges(api, edge):
+    b, orc = edge
+    pr = b.pr
+    pp = perturbed_jones(pr, seed=9)
+    want = orc.predict_full(pp)
+    with blib.DeviceProblem(api, pr.N, pr.Nbase, pr.tilesz, b.barr, b.sky, pr.coh, pr.x) as dp:
+        _, got = dp.predict(pp, out_mode=2)
+        c, res = dp.predict(pp, out_mode=1, cost_mode=1)
+    assert relerr(got, want) < 1e-13
+    assert relerr(res, pr.x - want) < 1e-13
+    assert abs(c - np.sum((pr.x - want) ** 2)) <= 1e-12 * c
+
+
+@pytest.mark.parametrize("robust", [False, True])
+def test_cost_and_grad_station_edges(api, edge, robust):
+    b, orc = edge
+    pr = b.pr
+    pp = perturbed_jones(pr, seed=5)
+    nu = 3.5
+    cw = orc.cost(pp, pr.x, robust=robust, nu=nu)
+    gw = orc.grad(pp, pr.x, robust=robust, nu=nu)
+    with blib.DeviceProblem(api, pr.N, pr.Nbase, pr.tilesz, b.barr, b.sky, pr.coh, pr.x) as dp:
+        c = dp.cost(pp, robust=robust, nu=nu)
+        g = dp.grad(pp, robust=robust, nu=nu)
+    assert abs(c - cw) <= 1e-12 * abs(cw)
+    assert relerr(g, gw) < 1e-11
+
+
+@pytest.mark.parametrize("weighted", [False, True])
+def test_normal_equations_station_edges(api, edge, weighted):
+    b, orc = edge
+    pr = b.pr
+    pp = perturbed_jones(pr, seed=7)
+    rng = np.random.default_rng(1)
+    xd = pr.x + 0.01 * rng.normal(0, 1, pr.x.shape)
+    xd.reshape(-1, 8)[pr.flag == 1] = 0.0
+    wt = rng.uniform(0.2, 1.3, pr.x.shape) if weighted else None
+    with blib.DeviceProblem(api, pr.N, pr.Nbase, pr.tilesz, b.barr, b.sky, pr.coh, pr.x) as dp:
+        off = 0
+        for k in range(pr.M):
+            for ck in range(pr.nchunk[k]):
+                pblk = pp[off:off + 8 * pr.N].copy()
+                off += 8 * pr.N
+                t0, nt = orc.chunk_tiles(k, ck)
+                if nt <= 0:
+                    continue
+                sl = slice(8 * t0 * pr.Nbase, 8 * (t0 + nt) * pr.Nbase)
+                cw, Aw, bw = orc.normal_eq(k, t0, nt, pblk, xd[sl], wt[sl] if weighted else None)
+                if weighted:
+                    c, JTJ, JTe = dp.normal_eq_weighted(k, ck, pblk, xd, wt)
+                else:
+                    c, JTJ, JTe = dp.normal_eq(k, ck, pblk, xd)
+                assert abs(c - cw) <= 1e-12 * cw, (k, ck)
+                assert relerr(JTe, bw) < 1e-11, (k, ck)
+                assert relerr(JTJ, Aw) < 1e-11, (k, ck)
