@@ -272,6 +272,8 @@ struct ClusterPassArgs {
   const double *pblk_old;    // mode 3 with beta != 1, instead of in2: the Jones the hidden data was
                              // formed with; the old residual is recovered as (d - f(p_old))/beta, so
                              // out = d - f(p) + (1-beta)/beta (d - f(p_old)) costs no extra traffic
+  int form_hidden;           // modes 1 and 3: `in` is the residual r and the hidden data is formed per
+                             // row as d = beta r + f(pblk_old), never stored (linear-mapped variant only)
   const short2 *blpq;        // [Nbase] (p,q) of baseline b (linear-mapped variant)
   double *jte_part;          // [groups][slices][8N] per-CTA station sums (linear-mapped variant)
   unsigned int *gcounter;    // [groups] arrival counters of the time slices of a baseline group
@@ -395,6 +397,9 @@ void db_launch_grad_full(const GradArgs *a, int ntile, cudaStream_t st);
 void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st);
 int db_cluster_pass_nblocks(int ntile, int nt, int tslice);
 void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st);
+// whether plain (unweighted) passes of this array take k_cluster_pass_lin, the one variant that
+// forms the hidden data itself (ClusterPassArgs::form_hidden)
+int db_cluster_pass_forms_hidden(int N, int Nbase);
 void db_launch_coh_gram(const GramArgs *a, int ntile, int nk, cudaStream_t st);
 void db_launch_assemble(const AssembleArgs *a, int ntile, cudaStream_t st);
 void db_launch_copy_add_diag(const double *A0, double *A, int n, double mu, cudaStream_t st);

@@ -1000,14 +1000,24 @@ k_cluster_pass_lin(ClusterPassArgs a) {
   for (int c = 0; c < 4; c++) Jq[c] = make_double2(0.0, 0.0);
   unsigned flagbits = 0;  // bit j: row ts+j flagged (slices are at most 32 rows, see the launcher)
   const long long b = b0 + bl;
-  // closing pass of a sharded visit: the old residual is recovered from the Jones the visit started
-  // with, out = d - f(p) + (1-beta)/beta (d - f(p_old))
-  const bool recover = (!GRAD) && a.mode == 3 && a.pblk_old != nullptr;
+  // A second model, at the Jones the visit started with (pblk_old):
+  //  * closing pass of a sharded visit (in = d): the old residual is recovered,
+  //    out = d - f(p) + (1-beta)/beta (d - f(p_old))
+  //  * form_hidden (in = r): the hidden data d = beta r + f(p_old) is formed per row, so that it
+  //    never has to be stored
+  const bool recover = (!GRAD) && a.mode == 3 && a.pblk_old != nullptr && !a.form_hidden;
+  const bool old_model = recover || a.form_hidden;
   const double gamma = recover ? (1.0 - a.beta) / a.beta : 0.0;
   double2 Jro[2], Jqo[4];
   Jro[0] = Jro[1] = make_double2(0.0, 0.0);
 #pragma unroll
   for (int c = 0; c < 4; c++) Jqo[c] = make_double2(0.0, 0.0);
+  auto load_old_jones = [&]() {
+    const double2 *jo = reinterpret_cast<const double2 *>(a.pblk_old + 8 * (long long)p + 4 * h);
+    Jro[0] = __ldg(jo);
+    Jro[1] = __ldg(jo + 1);
+    load_jones(a.pblk_old, q, Jqo);
+  };
   if (valid) {
     const short2 pq = a.blpq[b];
     p = pq.x;
@@ -1016,12 +1026,7 @@ k_cluster_pass_lin(ClusterPassArgs a) {
     Jr[0] = __ldg(jp);
     Jr[1] = __ldg(jp + 1);
     load_jones(a.pblk, q, Jq);
-    if (recover) {
-      const double2 *jo = reinterpret_cast<const double2 *>(a.pblk_old + 8 * (long long)p + 4 * h);
-      Jro[0] = __ldg(jo);
-      Jro[1] = __ldg(jo + 1);
-      load_jones(a.pblk_old, q, Jqo);
-    }
+    if (old_model && !GRAD) load_old_jones();
     for (int j = 0; j < nrow; j++)
       flagbits |= (a.flag[(long long)(ts + j) * a.Nbase + b] != 0 ? 1u : 0u) << j;
   }
@@ -1047,6 +1052,23 @@ k_cluster_pass_lin(ClusterPassArgs a) {
       m[0] = cdot2c(T0, Jq[0], T1, Jq[1]);
       m[1] = cdot2c(T0, Jq[2], T1, Jq[3]);
       if (fl) m[0] = m[1] = make_double2(0.0, 0.0);
+      double2 mo[2];
+      if (old_model) {
+        // next to the gradient accumulator the second Jones set does not fit in registers (it
+        // spills): it is read again for every row, from L1
+        if (GRAD) load_old_jones();
+        const double2 U0 = cdot2(Jro[0], C[0], Jro[1], C[2]);
+        const double2 U1 = cdot2(Jro[0], C[1], Jro[1], C[3]);
+        mo[0] = cdot2c(U0, Jqo[0], U1, Jqo[1]);
+        mo[1] = cdot2c(U0, Jqo[2], U1, Jqo[3]);
+        if (fl) mo[0] = mo[1] = make_double2(0.0, 0.0);
+      }
+      if (a.form_hidden) {
+        // the same rounded add as the INIT pass that would have stored d
+#pragma unroll
+        for (int jj = 0; jj < 2; jj++)
+          v[jj] = cadd(make_double2(a.beta * v[jj].x, a.beta * v[jj].y), mo[jj]);
+      }
       double2 e[2];
       if (a.mode == 0 || a.mode == 2) {
 #pragma unroll
@@ -1056,14 +1078,6 @@ k_cluster_pass_lin(ClusterPassArgs a) {
           e[jj] = csub(d, m[jj]);
         }
       } else {
-        double2 mo[2];
-        if (recover) {
-          const double2 U0 = cdot2(Jro[0], C[0], Jro[1], C[2]);
-          const double2 U1 = cdot2(Jro[0], C[1], Jro[1], C[3]);
-          mo[0] = cdot2c(U0, Jqo[0], U1, Jqo[1]);
-          mo[1] = cdot2c(U0, Jqo[2], U1, Jqo[3]);
-          if (fl) mo[0] = mo[1] = make_double2(0.0, 0.0);
-        }
 #pragma unroll
         for (int jj = 0; jj < 2; jj++) {
           e[jj] = csub(v[jj], m[jj]);
@@ -1315,12 +1329,28 @@ void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st) {
   }
 }
 int db_cluster_pass_nblocks(int ntile, int nt, int tslice) { return ntile * ((nt + tslice - 1) / tslice); }
+// the linear-mapped kernel keeps 8N station sums in shared memory next to its ring and one arrival
+// counter per 256-baseline group: arrays too large for either take the tile kernels
+static bool cluster_pass_lin_fits(int N, int Nbase) {
+  return (size_t)5 * 8 * 256 * sizeof(double2) + sizeof(double) * ((8 * N + 1) & ~1) + 40 <=
+             (size_t)200 * 1024 && (Nbase + 255) / 256 <= 1024;
+}
+int db_cluster_pass_forms_hidden(int N, int Nbase) {
+  static const bool tiles = getenv("DIRAC_B200_NO_TMA") != nullptr ||
+                            getenv("DIRAC_B200_CP_UNSPLIT") != nullptr ||
+                            getenv("DIRAC_B200_ADDSUB_TILE") != nullptr;
+  return !tiles && cluster_pass_lin_fits(N, Nbase);
+}
 void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st) {
   int nt = a->t_end - a->t_begin;
   dim3 grid(ntile, (nt + a->tslice - 1) / a->tslice);
+  if (a->form_hidden && (a->wt || a->in2 || !db_cluster_pass_forms_hidden(a->N, a->Nbase))) {
+    fprintf(stderr, "dirac_b200: cluster pass that forms the hidden data requested where only the tile "
+                    "kernels run (%s:%d)\n", __FILE__, __LINE__);
+    exit(1);
+  }
   static const bool no_tma_any = getenv("DIRAC_B200_NO_TMA") != nullptr;
-  const bool lin_ok = (size_t)5 * 8 * 256 * sizeof(double2) + sizeof(double) * ((8 * a->N + 1) & ~1) + 40 <=
-                          (size_t)200 * 1024 && (a->Nbase + 255) / 256 <= 1024;
+  const bool lin_ok = cluster_pass_lin_fits(a->N, a->Nbase);
   if (!(a->jte != nullptr && a->mode <= 1) && !a->wt && !a->in2 && !no_tma_any && lin_ok &&
       !getenv("DIRAC_B200_ADDSUB_TILE")) {
     // ADD / SUB / cost-only pass in the linear mapping: the same CTA-wide TMA ring as the gradient
@@ -1355,10 +1385,7 @@ void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st
     // default: linear mapping with CTA-wide TMA stages; robust weights and DIRAC_B200_NO_TMA take the
     // register-staged tile kernel
     static const bool no_tma = getenv("DIRAC_B200_NO_TMA") != nullptr;
-    // the linear-mapped kernel keeps 8N station sums in shared memory next to its ring and one
-    // arrival counter per 256-baseline group: arrays too large for either take the tile kernel
-    const bool lin_fits = (size_t)5 * 8 * 256 * sizeof(double2) + sizeof(double) * ((8 * a->N + 1) & ~1) + 40 <=
-                              (size_t)200 * 1024 && (a->Nbase + 255) / 256 <= 1024;
+    const bool lin_fits = cluster_pass_lin_fits(a->N, a->Nbase);
     if (unsplit) {
       k_cluster_pass<true><<<grid, TILE_THREADS, 0, st>>>(*a);
     } else if (a->wt || no_tma || !lin_fits) {

@@ -192,13 +192,14 @@ static int pick_tslice(const DevProblem &d, int nt) {
 void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
                      double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
                      int t1, const double2 *wt, double beta = 1.0, const double2 *in2 = nullptr,
-                     bool jte_zeroed = false, const double *pblk_old = nullptr);
+                     bool jte_zeroed = false, const double *pblk_old = nullptr,
+                     bool form_hidden = false);
 
 // one streaming pass of cluster k over timeslots [t0,t1): see ClusterPassArgs for the modes
 void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
                      double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
                      int t1, const double2 *wt, double beta, const double2 *in2, bool jte_zeroed,
-                     const double *pblk_old) {
+                     const double *pblk_old, bool form_hidden) {
   DevProblem &d = pr->d;
   if (t1 <= t0) {
     if (mode <= 1 || mode == 4)
@@ -213,7 +214,7 @@ void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, cons
   a.partials = pr->partials; a.cost = d.scal + cost_slot; a.counter = d.counters; a.R = d.R;
   a.N = d.N; a.Nbase = d.Nbase; a.t_begin = t0; a.t_end = t1; a.tslice = pick_tslice(d, t1 - t0);
   a.mode = mode; a.write_out = write_out; a.wt = wt; a.beta = beta; a.in2 = in2;
-  a.pblk_old = pblk_old;
+  a.pblk_old = pblk_old; a.form_hidden = form_hidden;
   // passes without the gradient accumulator fit two CTAs per SM: twice as many, half as long
   if (!(jte_dev && (mode <= 1 || mode == 4)) && g_tslice_override <= 0 && a.tslice > 1)
     a.tslice = (a.tslice + 1) / 2;
@@ -523,8 +524,12 @@ void db_prefactor_sweep(dirac_b200_problem *pr, double tau) {
 
 // ------------------------------------------------------------------------------------------------
 // the LM iteration loop shared by the four reference variants.  On entry the hidden data of the
-// chunk is in w.dbuf and pblk_dev holds p.  If `have_first` the caller already produced
-// ||e||^2 (in *first_cost) and J^T e (in w.JTe) at p with the same weights (the fused first pass).
+// chunk is in w.dbuf and pblk_dev holds p, or, if `hidden_from` is given, the trial passes form the
+// hidden data per row from that residual and the entry Jones in w.pold; the trial of the last
+// iteration then writes its residual d - f(p_trial) into w.dbuf (LmOut::res_in_dbuf: that trial
+// was accepted, w.dbuf holds the residual at the final Jones).  If `have_first` the caller already
+// produced ||e||^2 (in *first_cost) and J^T e (in w.JTe) at p with the same weights (the fused first
+// pass).
 // wt == null: plain LM, J^T J from the cached Gram tensor; wt != null: robust LM round.
 // `nu_damp` is the integer damping multiplier that the robust driver carries across its IRLS rounds
 // (robustlm.c keeps `nu` alive over the nw loop).  `evaluated_trial` reports whether w.plast holds
@@ -580,12 +585,13 @@ extern "C" void db_launch_lm_aug_rhs(double *jte, const double *p, const double 
 struct LmOut {
   double init_eL2, eL2, jacTe_inf, Dp_L2, mu;
   int k, stop;
+  bool res_in_dbuf;
 };
 
 static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, double *pblk_dev,
                     const double2 *wt, int itmax, const double *opts, int linsolv, int os,
                     int os_shift, int randomize, bool have_first, double first_cost, int *nu_damp,
-                    bool *evaluated_trial, LmOut *out) {
+                    bool *evaluated_trial, const double2 *hidden_from, LmOut *out) {
   DevProblem &d = pr->d;
   LMWork &w = pr->lm;
   const int n = w.n8;
@@ -640,6 +646,7 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
   int nu = *nu_damp, nu2;
   double mu = 0.0, Dp_L2 = DBL_MAX, jacTe_inf = 0.0;
   *evaluated_trial = false;
+  bool res_in_dbuf = false;
   bool pending_entry = defer;  // entry values not on the host yet
   w.jtj_spec = nullptr;
   int kiter_adjust = 0;
@@ -848,8 +855,17 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
         if (!w.step_fused)
           db_launch_lm_step(pblk_dev, w.Dp, w.JTe, w.pnew, d.scal + 8, os ? nullptr : w.JTe_new, n,
                             d.stream);
-        db_cluster_pass(pr, k, w.pnew, w.dbuf, nullptr, 1, 0, os ? nullptr : w.JTe_new, 1, t0, t1,
-                        wt, 1.0, nullptr, true);
+        if (hidden_from) {
+          // the last iteration ends with this trial if it is accepted: its J^T e would never be read,
+          // its residual is the one the visit leaves behind
+          const bool last = kiter == itmax - 1;
+          db_cluster_pass(pr, k, w.pnew, hidden_from, last ? w.dbuf : nullptr, 1, last ? 1 : 0,
+                          last ? nullptr : w.JTe_new, 1, t0, t1, nullptr, 1.0, nullptr, true, w.pold,
+                          true);
+        } else {
+          db_cluster_pass(pr, k, w.pnew, w.dbuf, nullptr, 1, 0, os ? nullptr : w.JTe_new, 1, t0, t1,
+                          wt, 1.0, nullptr, true);
+        }
         if (aug)
           db_launch_lm_aug_rhs(w.JTe_new, w.pnew, aug->y_dev, aug->bz_dev, aug->rho, n, d.stream);
         if (!w.step_fused) db_count_launch(1);  // k_lm_step
@@ -951,6 +967,7 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
             }
             p_eL2 = pDp_eL2;
             w.jtj_spec = spec_buf;
+            res_in_dbuf = hidden_from && kiter == itmax - 1;
             break;
           }
         }
@@ -976,6 +993,7 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
   out->mu = mu;
   out->k = kiter;
   out->stop = stop;
+  out->res_in_dbuf = res_in_dbuf;
 }
 
 static void fill_info(double *info, const LmOut &o) {
@@ -1018,7 +1036,7 @@ void db_lm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, double
     bool ev;
     LmOut o;
     lm_core(pr, k, ck, t0, t1, pblk_dev, nullptr, itmax, opts ? opts : defopts, linsolv, os, 0,
-            randomize, false, 0.0, &nu, &ev, &o);
+            randomize, false, 0.0, &nu, &ev, nullptr, &o);
     fill_info(info, o);
     return;
   }
@@ -1026,10 +1044,18 @@ void db_lm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, double
   // the first func/jacf evaluation, clmfit.c:241-252)
   // (sharded runs weight the residual share of the hidden data with beta, SAGE: d = f + beta r)
   const double beta = pr->world > 1 ? pr->beta : 1.0;
-  if (beta != 1.0)  // the closing pass recovers the old residual from the Jones the visit started with
+  // A plain LM visit of a one-chunk cluster never stores the hidden data: every pass forms it again
+  // from r and the entry Jones (w.pold), which costs no traffic, and the trial of the last iteration
+  // writes the residual, so that the closing pass is only needed when the visit ends otherwise.  A
+  // cluster of several chunks keeps d: the last trial covers only the chunk's rows of the residual.
+  const bool form = !os && pr->world <= 1 && d.h_clus[k].nchunk == 1 && r == pr->res &&
+                    db_cluster_pass_forms_hidden(d.N, d.Nbase);
+  // the sharded closing pass recovers the old residual from the Jones the visit started with
+  if (beta != 1.0 || form)
     DB_CHECK(cudaMemcpyAsync(w.pold, pblk_dev, sizeof(double) * w.n8, cudaMemcpyDeviceToDevice,
                              d.stream));
-  db_cluster_pass(pr, k, pblk_dev, r, w.dbuf, 0, 1, os ? nullptr : w.JTe, 2, t0, t1, nullptr, beta);
+  db_cluster_pass(pr, k, pblk_dev, r, form ? nullptr : w.dbuf, 0, form ? 0 : 1,
+                  os ? nullptr : w.JTe, 2, t0, t1, nullptr, beta);
   // ||e||^2 at entry stays on the device for now: lm_core fetches it together with p and J^T e
   // (NaN = "still in d.scal[2]")
   const double c0 = nan("");
@@ -1037,11 +1063,19 @@ void db_lm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, double
   bool ev;
   LmOut o;
   lm_core(pr, k, ck, t0, t1, pblk_dev, nullptr, itmax, opts ? opts : defopts, linsolv, os, 0,
-          randomize, true, c0, &nu, &ev, &o);
+          randomize, true, c0, &nu, &ev, form ? r : nullptr, &o);
   // residual of the chunk with the final Jones: r = d - f(p) (+ (1-beta) r when sharded)
   // (lmfit.c:980-981)
-  db_cluster_pass(pr, k, pblk_dev, w.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta, nullptr, false,
-                  beta != 1.0 ? w.pold : nullptr);
+  if (o.res_in_dbuf) {
+    pr->res = w.dbuf;
+    w.dbuf = r;
+  } else if (form) {
+    db_cluster_pass(pr, k, pblk_dev, r, r, 3, 1, nullptr, 1, t0, t1, nullptr, 1.0, nullptr, false,
+                    w.pold, true);
+  } else {
+    db_cluster_pass(pr, k, pblk_dev, w.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta, nullptr,
+                    false, beta != 1.0 ? w.pold : nullptr);
+  }
   fill_info(info, o);
 }
 
@@ -1140,7 +1174,7 @@ void db_rlm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
   for (int nw = 0; nw < wt_itmax; nw++) {
     bool evaluated = false;
     lm_core(pr, k, ck, t0, t1, pblk_dev, w.wbuf, itmax, defopts, linsolv, os, nw, randomize, false,
-            0.0, &nu, &evaluated, &o);
+            0.0, &nu, &evaluated, nullptr, &o);
     if (nw < wt_itmax - 1 && r1 > r0) {
       // residual the new weights are computed from: at nw == 0 the reference's `ed` is the
       // (unit-weight) residual of the LAST evaluated point, which is a rejected trial if the loop

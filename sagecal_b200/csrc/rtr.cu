@@ -21,7 +21,7 @@
 void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
                      double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
                      int t1, const double2 *wt, double beta, const double2 *in2, bool jte_zeroed,
-                     const double *pblk_old);
+                     const double *pblk_old, bool form_hidden = false);
 void db_chunk_range(const DevProblem &d, int k, int ck, int *t0, int *t1);
 
 struct RtrWork {

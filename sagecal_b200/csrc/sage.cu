@@ -86,8 +86,9 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
 
   DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * m, cudaMemcpyHostToDevice, d.stream));
   // residual of the current model: r = x - sum_k model_k, res_0 = ||r|| / n   (lmfit.c:866-869)
-  double2 *r = pr->res;
-  db_predict_dev(pr, d.pp, r, 1, 1, 0.0, 0);
+  // (r is pr->res, read afresh where it is used: an LM visit may hand back its residual in another
+  // buffer, lm.cu db_lm_chunk)
+  db_predict_dev(pr, d.pp, pr->res, 1, 1, 0.0, 0);
   *res_0 = sqrt(db_read_scalar(pr, 0)) / (double)n;
 
   int weighted_iter = 0;
@@ -96,7 +97,7 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
   for (int ci = 0; ci < max_emiter; ci++) {
     if (sharded) {
       // remember the state every rank starts the sweep from
-      DB_CHECK(cudaMemcpyAsync(pr->pm, r, sizeof(double2) * 4 * d.R, cudaMemcpyDeviceToDevice,
+      DB_CHECK(cudaMemcpyAsync(pr->pm, pr->res, sizeof(double2) * 4 * d.R, cudaMemcpyDeviceToDevice,
                                d.stream));
       DB_CHECK(cudaMemcpyAsync(pr->pp_start, d.pp, sizeof(double) * m, cudaMemcpyDeviceToDevice,
                                d.stream));
@@ -124,7 +125,7 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
         // hybrid chunks that do not tile the interval evenly: hidden data and residual of the whole
         // cluster with the reference's row-based chunk map, the LM fits in between
         const bool hr = db_cluster_needs_rowmap(pr, cj);
-        if (hr) db_cluster_hidden(pr, cj, r, +1);
+        if (hr) db_cluster_hidden(pr, cj, pr->res, +1);
         for (int ck = 0; ck < hc[cj].nchunk; ck++) {
           const int poff = d.h_chunk_poff[hc[cj].chunk0 + ck];
           double *pblk = d.pp + poff;
@@ -133,8 +134,8 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
             // ADMM J-update as the reference does it (admm_solve.c:331-352): robust RTR on the
             // consensus-augmented cost, whatever solver_mode the caller named
             if (!ci) rtr_nu = robust_nu0;
-            db_rtr_chunk(pr, cj, ck, pblk, r, 5, this_itermax + 5, this_itermax + 10, nulow, nuhigh,
-                         &rtr_nu, info, hr, pr->aug_y_host + poff, pr->aug_bz_host + poff,
+            db_rtr_chunk(pr, cj, ck, pblk, pr->res, 5, this_itermax + 5, this_itermax + 10, nulow,
+                         nuhigh, &rtr_nu, info, hr, pr->aug_y_host + poff, pr->aug_bz_host + poff,
                          pr->aug_rho[cg]);
             if (last) robust_nuM[cg] += rtr_nu;
             init_res += info[0];
@@ -145,50 +146,53 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
             db_lm_set_aug(pr->aug_dev + poff, pr->aug_dev + d.npar + poff, pr->aug_y_host + poff,
                           pr->aug_bz_host + poff, pr->aug_rho[cg]);
           if (solver_mode == SM_OSLM_LBFGS) {
-            db_lm_chunk(pr, cj, ck, pblk, r, this_itermax, opts, linsolv, last ? 0 : 1, randomize,
-                        info, hr);
+            db_lm_chunk(pr, cj, ck, pblk, pr->res, this_itermax, opts, linsolv, last ? 0 : 1,
+                        randomize, info, hr);
           } else if (solver_mode == SM_LM_LBFGS) {
-            db_lm_chunk(pr, cj, ck, pblk, r, this_itermax, opts, linsolv, 0, randomize, info, hr);
+            db_lm_chunk(pr, cj, ck, pblk, pr->res, this_itermax, opts, linsolv, 0, randomize, info,
+                        hr);
           } else if (solver_mode == SM_RLM_RLBFGS) {
             if (last) {
               double nu = robust_nu0;
-              db_rlm_chunk(pr, cj, ck, pblk, r, this_itermax, linsolv, 0, randomize, nulow, nuhigh,
-                           &nu, info, hr);
+              db_rlm_chunk(pr, cj, ck, pblk, pr->res, this_itermax, linsolv, 0, randomize, nulow,
+                           nuhigh, &nu, info, hr);
               robust_nuM[cg] += nu;
             } else {
-              db_lm_chunk(pr, cj, ck, pblk, r, this_itermax, opts, linsolv, 1, randomize, info, hr);
+              db_lm_chunk(pr, cj, ck, pblk, pr->res, this_itermax, opts, linsolv, 1, randomize,
+                          info, hr);
             }
           } else if (solver_mode == SM_RTR_OSLM_LBFGS) {
             // RSD + RTR (lmfit.c:934-937)
-            db_rtr_chunk(pr, cj, ck, pblk, r, 4, this_itermax + 5, this_itermax + 10, nulow,
+            db_rtr_chunk(pr, cj, ck, pblk, pr->res, 4, this_itermax + 5, this_itermax + 10, nulow,
                          nuhigh, &rtr_nu, info, hr, nullptr, nullptr, 0.0);
           } else if (solver_mode == SM_RTR_OSRLM_RLBFGS) {
             // robust RTR; nu persists from visit to visit after the first sweep (lmfit.c:938-947)
             if (!ci) rtr_nu = robust_nu0;
-            db_rtr_chunk(pr, cj, ck, pblk, r, 5, this_itermax + 5, this_itermax + 10, nulow,
+            db_rtr_chunk(pr, cj, ck, pblk, pr->res, 5, this_itermax + 5, this_itermax + 10, nulow,
                          nuhigh, &rtr_nu, info, hr, nullptr, nullptr, 0.0);
             if (last) robust_nuM[cg] += rtr_nu;
           } else if (solver_mode == SM_NSD_RLBFGS) {
             // Nesterov's accelerated descent (lmfit.c:948-957)
             if (!ci) rtr_nu = robust_nu0;
-            db_rtr_chunk(pr, cj, ck, pblk, r, 6, this_itermax + 15, 0, nulow, nuhigh, &rtr_nu,
+            db_rtr_chunk(pr, cj, ck, pblk, pr->res, 6, this_itermax + 15, 0, nulow, nuhigh, &rtr_nu,
                          info, hr, nullptr, nullptr, 0.0);
             if (last) robust_nuM[cg] += rtr_nu;
           } else {  // SM_OSLM_OSRLM_RLBFGS
             if (last) {
               double nu = robust_nu0;
-              db_rlm_chunk(pr, cj, ck, pblk, r, this_itermax, linsolv, 1, randomize, nulow, nuhigh,
-                           &nu, info, hr);
+              db_rlm_chunk(pr, cj, ck, pblk, pr->res, this_itermax, linsolv, 1, randomize, nulow,
+                           nuhigh, &nu, info, hr);
               robust_nuM[cg] += nu;
             } else {
-              db_lm_chunk(pr, cj, ck, pblk, r, this_itermax, opts, linsolv, 1, randomize, info, hr);
+              db_lm_chunk(pr, cj, ck, pblk, pr->res, this_itermax, opts, linsolv, 1, randomize,
+                          info, hr);
             }
           }
           init_res += info[0];
           final_res += info[1];
           if (pr->aug_rho) db_lm_set_aug(nullptr, nullptr, nullptr, nullptr, 0.0);
         }
-        if (hr) db_cluster_hidden(pr, cj, r, -1);
+        if (hr) db_cluster_hidden(pr, cj, pr->res, -1);
         if (init_res > 0.0) {
           nerr[cg] = (init_res - final_res) / init_res;
           if (nerr[cg] < 0.0) nerr[cg] = 0.0;
@@ -204,7 +208,8 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
       double *xb = pr->xb;
       double2 *xr = reinterpret_cast<double2 *>(xb);
       double2 *xp = reinterpret_cast<double2 *>(xb + (size_t)8 * d.R);
-      DB_CHECK(cudaMemcpyAsync(xr, r, sizeof(double2) * 4 * d.R, cudaMemcpyDeviceToDevice, d.stream));
+      DB_CHECK(cudaMemcpyAsync(xr, pr->res, sizeof(double2) * 4 * d.R, cudaMemcpyDeviceToDevice,
+                               d.stream));
       db_launch_axpby(pr->pm, xr, 4 * d.R, -1.0, 1.0, d.stream);
       DB_CHECK(cudaMemcpyAsync(xp, d.pp, sizeof(double) * m, cudaMemcpyDeviceToDevice, d.stream));
       db_launch_axpby(reinterpret_cast<double2 *>(pr->pp_start), xp, m / 2, -1.0, 1.0, d.stream);
@@ -213,9 +218,9 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
       db_allreduce(pr, xb, (long long)xb_len);
       DB_CHECK(cudaMemcpyAsync(nerr.data(), xb + (size_t)8 * d.R + m, sizeof(double) * MG,
                                cudaMemcpyDeviceToHost, d.stream));
-      DB_CHECK(cudaMemcpyAsync(r, pr->pm, sizeof(double2) * 4 * d.R, cudaMemcpyDeviceToDevice,
+      DB_CHECK(cudaMemcpyAsync(pr->res, pr->pm, sizeof(double2) * 4 * d.R, cudaMemcpyDeviceToDevice,
                                d.stream));
-      db_launch_axpby(xr, r, 4 * d.R, 1.0, 1.0, d.stream);
+      db_launch_axpby(xr, pr->res, 4 * d.R, 1.0, 1.0, d.stream);
       DB_CHECK(cudaMemcpyAsync(d.pp, pr->pp_start, sizeof(double) * m, cudaMemcpyDeviceToDevice,
                                d.stream));
       db_launch_axpby(xp, reinterpret_cast<double2 *>(d.pp), m / 2, 1.0, 1.0, d.stream);
@@ -254,9 +259,9 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
   }
   // final residual, in place in x   (lmfit.c:1039-1044)
   DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * m, cudaMemcpyHostToDevice, d.stream));
-  db_predict_dev(pr, d.pp, r, 1, 1, 0.0, 0);
+  db_predict_dev(pr, d.pp, pr->res, 1, 1, 0.0, 0);
   *res_1 = sqrt(db_read_scalar(pr, 0)) / (double)n;
-  if (x_out) db_download_vis(pr, r, x_out);
+  if (x_out) db_download_vis(pr, pr->res, x_out);
   *mean_nu = robust_nu0;
   DB_CHECK(cudaGetLastError());
   return (*res_1 > *res_0) ? -1 : 0;
