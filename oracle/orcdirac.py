@@ -78,6 +78,11 @@ class Oracle:
             self.HT.harness_rtr_solve_tensor.argtypes = [pp, i, i, i, dp, i, dp, i, i, d, d, dp, dp,
                                                          i, dp, dp, d]
             self.HT.harness_rtr_solve_tensor.restype = None
+        L.orc_rtr_raw.restype = d
+        L.orc_rtr_raw.argtypes = [pp, i, i, i, dp, dp, dp, dp, dp]
+        L.orc_rtr_counts.argtypes = [pp, i, i, dp]
+        L.orc_rtr_weights.restype = d
+        L.orc_rtr_weights.argtypes = [pp, i, i, i, dp, dp, d, dp]
         L.orc_generate_baselines.argtypes = [i, i, i, ip, ip]
         L.orc_preset_flags_and_data.argtypes = [i, dp, up, dp]
         ps = C.POINTER(orc_sky)
@@ -180,6 +185,31 @@ class Oracle:
                                       _d(xd), kind, _d(p), itmax_a, itmax_b, nulow, nuhigh,
                                       C.byref(nu), _d(info), int(nu_joined), yp, zp, rho)
         return p, info, nu.value
+
+    # ---- the per-row RTR evaluators (orc_rtr_*) on hidden data y of tiles [t0, t0 + ntiles) ----
+    def rtr_raw(self, k, t0, ntiles, y, x, eta=None, wt=None, vec=True):
+        """(cost, raw station sums [8N] or None): gradient sums (eta None) or Hessian terms"""
+        y = np.ascontiguousarray(y, dtype=np.float64)
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        v = np.zeros(8 * self.pr.N) if vec else None
+        e = None if eta is None else np.ascontiguousarray(eta, dtype=np.float64)
+        w = None if wt is None else np.ascontiguousarray(wt, dtype=np.float64)
+        c = self.L.orc_rtr_raw(C.byref(self.P), k, t0, ntiles, _d(y), _d(w) if w is not None else None,
+                               _d(x), _d(e) if e is not None else None, _d(v) if vec else None)
+        return c, v
+
+    def rtr_counts(self, t0, ntiles):
+        c = np.zeros(self.pr.N)
+        self.L.orc_rtr_counts(C.byref(self.P), t0, ntiles, _d(c))
+        return c
+
+    def rtr_weights(self, k, t0, ntiles, y, x, nu):
+        """(sum(log w - w) over unflagged rows / all rows, row weights; flagged rows 0)"""
+        y = np.ascontiguousarray(y, dtype=np.float64)
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        wt = np.zeros(ntiles * self.pr.Nbase)
+        s = self.L.orc_rtr_weights(C.byref(self.P), k, t0, ntiles, _d(y), _d(x), nu, _d(wt))
+        return s, wt
 
     def update_w_and_nu(self, nu0, ed, nulow=2.0, nuhigh=30.0):
         w = np.zeros(len(ed))

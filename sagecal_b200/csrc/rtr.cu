@@ -94,6 +94,9 @@ struct RtrDevEval {
   int k, t0, t1, N, n8;
   long long nrows;            // rows of the chunk, flagged ones included (the reference's M)
   std::vector<double> x_on_dev;  // the Jones w->xdev holds (empty: unknown)
+  bool force_dev = false;     // Jones through device memory at any N (test hook only)
+  int last_ns = 0, last_tslice = 0;  // time slicing of the last condensation
+  bool last_inline = false;          // the last evaluation had its vectors in the parameter block
 
   // condense the rows of the chunk.  xw != null: Student's-t row weights at xw with nu; returns
   // sum(log w - w) then
@@ -116,6 +119,8 @@ struct RtrDevEval {
     int ns = w->nslice < nt ? w->nslice : nt;
     a.tslice = (nt + ns - 1) / ns;
     ns = (nt + a.tslice - 1) / a.tslice;
+    last_ns = ns;
+    last_tslice = a.tslice;
     a.TD = ns > 1 ? w->TDpart : w->TD;
     a.sc = ns > 1 ? w->scpart : w->sc;
     a.tensors = tensors ? 1 : 0;
@@ -154,7 +159,8 @@ struct RtrDevEval {
   void launch(const double *x, const double *eta, double *fcost, double *vec, double *cnt) {
     DevProblem &d = pr->d;
     // results come back through the mailbox: no device-to-host copy, no stream synchronisation
-    const bool inl = N <= RTR_INLINE_MAXN;
+    const bool inl = N <= RTR_INLINE_MAXN && !force_dev;
+    last_inline = inl;
     RtrEvalInl P;
     RtrEvalArgs &a = P.a;
     a.TD = w->TD; a.sc = w->sc; a.x = w->xdev; a.eta = eta ? w->edev : nullptr;
@@ -258,4 +264,60 @@ void db_rtr_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
     db_cluster_pass(pr, k, pblk_dev, lw.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta, nullptr,
                     false, beta != 1.0 ? lw.pold : nullptr);
   db_stream_sync(d.stream);  // w->h is reused by the next visit
+}
+
+// test hook: the device evaluator of cluster k, chunk ck, exactly as a solver visit drives it (same
+// condense, same launch, same mailbox).  The hidden data of the chunk are the problem's data vector
+// (dirac_b200_set_data) as they stand, copied into the visit's hidden-data buffer.
+//   xw        null: unit weights; else Student's-t row weights at xw with nu (weights_at), `keep`
+//             selects whether they apply to the evaluations (the tensors are rebuilt) or only the
+//             scalars (sum(log w - w), unflagged rows) are condensed
+//   force_dev Jones and tangent vectors through device memory at any N
+//   ops[i]    evaluation i (host vectors x + 8N i, eta + 8N i): RTR_HOOK_* bits.  COUNTS alone is the
+//             evaluator's counts(); otherwise one launch with the requested outputs
+//   out       cost[neval], vec[neval][8N], cnt[neval][N]
+//   info      [sum(log w - w) / rows (0 for unit weights), nslice, tslice] of the condensation,
+//             [3] 1 if the last evaluation had its vectors in the parameter block
+enum { RTR_HOOK_COST = 1, RTR_HOOK_VEC = 2, RTR_HOOK_COUNTS = 4, RTR_HOOK_ETA = 8,
+       RTR_HOOK_UNIT = 16 };
+extern "C" void dirac_b200_rtr_eval(dirac_b200_problem *pr, int k, int ck, const double *xw,
+                                    double nu, int keep, int force_dev, int neval, const int *ops,
+                                    const double *x, const double *eta, double *cost, double *vec,
+                                    double *cnt, double *info) {
+  DevProblem &d = pr->d;
+  db_lm_init(pr);
+  RtrWork *w = rtr_init(pr);
+  int t0, t1;
+  db_chunk_range(d, k, ck, &t0, &t1);
+  if (t1 <= t0) {
+    fprintf(stderr, "dirac_b200_rtr_eval: chunk %d of cluster %d is empty\n", ck, k);
+    exit(1);
+  }
+  const int n8 = 8 * d.N;
+  DB_CHECK(cudaMemcpyAsync(pr->lm.dbuf, d.x, sizeof(double2) * 4 * d.R, cudaMemcpyDeviceToDevice,
+                           d.stream));
+  RtrDevEval E;
+  E.pr = pr; E.w = w; E.k = k; E.t0 = t0; E.t1 = t1; E.N = d.N; E.n8 = n8;
+  E.nrows = (long long)(t1 - t0) * d.Nbase;
+  E.force_dev = force_dev != 0;
+  info[0] = 0.0;
+  if (xw) info[0] = E.weights_at(xw, nu, keep != 0);
+  else E.unit_weights();
+  info[1] = E.last_ns;
+  info[2] = E.last_tslice;
+  for (int i = 0; i < neval; i++) {
+    const int op = ops[i];
+    if (op & RTR_HOOK_UNIT) E.unit_weights();
+    if ((op & ~RTR_HOOK_UNIT) == RTR_HOOK_COUNTS) {
+      E.counts(cnt + (size_t)i * d.N);
+      continue;
+    }
+    E.launch(x + (size_t)i * n8, (op & RTR_HOOK_ETA) ? eta + (size_t)i * n8 : nullptr,
+             (op & RTR_HOOK_COST) ? cost + i : nullptr,
+             (op & RTR_HOOK_VEC) ? vec + (size_t)i * n8 : nullptr,
+             (op & RTR_HOOK_COUNTS) ? cnt + (size_t)i * d.N : nullptr);
+  }
+  info[3] = E.last_inline ? 1.0 : 0.0;
+  db_stream_sync(d.stream);
+  DB_CHECK(cudaGetLastError());
 }

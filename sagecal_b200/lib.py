@@ -206,6 +206,48 @@ class DeviceProblem:
         return dict(E0=E[:self.n], E1=E[self.n:2 * self.n], E2=E[2 * self.n:], poly=poly,
                     cost_gauss=costs[0::2], cost_robust=costs[1::2], res=res, shape=tuple(shape))
 
+    #: operation bits of one rtr_eval evaluation (rtr.cu: RTR_HOOK_*)
+    RTR_COST, RTR_VEC, RTR_COUNTS, RTR_ETA, RTR_UNIT = 1, 2, 4, 8, 16
+
+    def rtr_eval(self, k, ck, evals, xw=None, nu=2.0, keep=True, force_device=False):
+        """the RTR device evaluator of cluster k, chunk ck on the data vector as hidden data
+        (dirac_b200_rtr_eval): one condensation (unit weights, or Student's-t weights at xw with nu;
+        keep=False condenses the scalars only), then `evals` in order, each a dict with x [8N] and
+        optional eta [8N], cost / vec / counts / unit (unit_weights() first) flags.
+        returns dict(results=[dict(cost, vec, counts) per evaluation, None where not asked],
+        slw [sum(log w - w) / rows], nslice, tslice, inline)"""
+        L = self.api.lib
+        L.dirac_b200_rtr_eval.restype = None
+        L.dirac_b200_rtr_eval.argtypes = [C.c_void_p, C.c_int, C.c_int, c_double_p, C.c_double,
+                                          C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), c_double_p,
+                                          c_double_p, c_double_p, c_double_p, c_double_p, c_double_p]
+        n8, ne = 8 * self.N, len(evals)
+        ops = np.zeros(ne, dtype=np.int32)
+        X = np.zeros((ne, n8))
+        ETA = np.zeros((ne, n8))
+        for i, e in enumerate(evals):
+            X[i] = e["x"]
+            if e.get("eta") is not None:
+                ETA[i] = e["eta"]
+                ops[i] |= self.RTR_ETA
+            ops[i] |= ((self.RTR_COST if e.get("cost") else 0) | (self.RTR_VEC if e.get("vec") else 0)
+                       | (self.RTR_COUNTS if e.get("counts") else 0)
+                       | (self.RTR_UNIT if e.get("unit") else 0))
+        cost = np.zeros(ne)
+        vec = np.zeros((ne, n8))
+        cnt = np.zeros((ne, self.N))
+        info = np.zeros(4)
+        xw_arr = None if xw is None else np.ascontiguousarray(xw, dtype=np.float64)
+        L.dirac_b200_rtr_eval(self.h, k, ck, dptr(xw_arr) if xw_arr is not None else None, nu,
+                              1 if keep else 0, 1 if force_device else 0, ne,
+                              ops.ctypes.data_as(C.POINTER(C.c_int)), dptr(X), dptr(ETA), dptr(cost),
+                              dptr(vec), dptr(cnt), dptr(info))
+        res = [dict(cost=cost[i] if ops[i] & self.RTR_COST else None,
+                    vec=vec[i] if ops[i] & self.RTR_VEC else None,
+                    counts=cnt[i] if ops[i] & self.RTR_COUNTS else None) for i in range(ne)]
+        return dict(results=res, slw=info[0], nslice=int(info[1]), tslice=int(info[2]),
+                    inline=bool(info[3]))
+
     def normal_eq(self, clus, chunk, pblk, xd):
         n8 = 8 * self.N
         JTJ = np.zeros((n8, n8))

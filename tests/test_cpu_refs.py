@@ -4,7 +4,8 @@ import numpy as np
 import pytest
 
 import orcdirac
-from util import big_cluster_sky, line_model_ref, relerr, small_problem, split_cluster
+from util import (big_cluster_sky, line_model_ref, relerr, rtr_eval_ref, rtr_weights_ref,
+                  small_problem, split_cluster)
 
 needs_oracle = pytest.mark.skipif(not orcdirac.available(), reason="oracle/liboracle.so not built")
 
@@ -23,6 +24,81 @@ def test_line_model_reference_is_the_model_along_the_line(nchunk):
     for a in (0.0, 0.7, -2.5):
         assert relerr(V0 + a * V1 + a * a * V2, orc.predict_full(xk + a * pk)) < 1e-14
     assert np.abs(V2).max() > 1e-3 * np.abs(V0).max()   # the quadratic term is not negligible
+
+
+def _rtr_case(flags, seed):
+    """an 11-station problem with a hybrid cluster whose second chunk starts at t0 > 0"""
+    b = small_problem(N=11, M=2, tilesz=7, seed=seed, nchunk=[1, 2], flag_frac=0.2, uvcut_frac=0.03)
+    pr = b.pr
+    if flags:   # one baseline flagged in every slot, one station with every row flagged
+        pr.flag[(pr.sta1 == 2) & (pr.sta2 == 5)] = 1
+        pr.flag[(pr.sta1 == 7) | (pr.sta2 == 7)] = 1
+    rng = np.random.default_rng(seed)
+    n8 = 8 * pr.N
+    x = pr.jones_true[:n8] + 0.05 * rng.normal(0, 1, n8)
+    e1, e2 = rng.normal(0, 0.1, n8), rng.normal(0, 0.1, n8)
+    return b, x, e1, e2
+
+
+def _assert_vec(got, want, scale, tol):
+    err = np.abs(np.asarray(got) - want).reshape(-1, 8).max(axis=1)
+    bound = tol * scale.reshape(-1, 8).max(axis=1)
+    assert (err <= bound).all(), (err / np.maximum(bound, 1e-300)).max()
+
+
+@needs_oracle
+@pytest.mark.parametrize("flags", [False, True], ids=["plain", "flagged"])
+def test_rtr_eval_reference_matches_oracle(flags):
+    """the numpy restatement of the RTR evaluator against the oracle's per-row evaluators
+    (orc_rtr_raw / _counts / _weights) on both chunks of a hybrid cluster, unit and Student's-t weights"""
+    b, x, e1, _ = _rtr_case(flags, 82)
+    pr = b.pr
+    orc = orcdirac.Oracle(pr)
+    n8 = 8 * pr.N
+    for k, ck in ((0, 0), (1, 0), (1, 1)):
+        t0, nt = orc.chunk_tiles(k, ck)
+        y = pr.x[8 * t0 * pr.Nbase:8 * (t0 + nt) * pr.Nbase]
+        xk = x + 0.01 * k
+        xw = xk + 0.02 * np.random.default_rng(k).normal(0, 1, n8)
+        cnt = orc.rtr_counts(t0, nt)
+        for nu in (None, 2.0, 30.0):
+            wt = None
+            if nu is not None:
+                s_orc, wt_orc = orc.rtr_weights(k, t0, nt, y, xw, nu)
+                slw, wt, slw_scale = rtr_weights_ref(pr, k, t0, nt, xw, nu)
+                assert abs(slw - s_orc) <= 1e-13 * slw_scale
+                assert relerr(wt, np.where(wt_orc > 0, wt_orc, 0.0)) < 1e-14
+            for eta in (None, e1):
+                c_orc, v_orc = orc.rtr_raw(k, t0, nt, y, xk, eta=eta, wt=wt)
+                r = rtr_eval_ref(pr, k, t0, nt, xk, eta=eta, wt=wt)
+                assert abs(r["cost"] - c_orc) <= 1e-13 * r["cost_scale"]
+                _assert_vec(r["vec"], v_orc, r["vec_scale"], 1e-13)
+                assert np.array_equal(r["counts"], cnt)
+        if flags:
+            assert cnt[7] == 0 and cnt.min() == 0 and cnt.max() > 0
+
+
+@pytest.mark.parametrize("weighted", [False, True], ids=["unit", "student-t"])
+def test_rtr_eval_reference_is_the_derivative_of_the_cost(weighted):
+    """calculus, no other code: d/dt cost(x + t eta) = -2 vec(x) . eta and d/dt vec(x + t eta) =
+    hess(x, eta).  The cost is a quartic and vec a cubic in t: both are fitted exactly from 5 points."""
+    b, x, e1, e2 = _rtr_case(True, 83)
+    pr = b.pr
+    k, t0, nt = 1, 4, 3
+    wt = rtr_weights_ref(pr, k, t0, nt, x + 0.03, 5.0)[1] if weighted else None
+    ts = np.array([-1.0, -0.5, 0.0, 0.5, 1.0])
+    r0 = rtr_eval_ref(pr, k, t0, nt, x, wt=wt)
+    for eta in (e1, e2):
+        rs = [rtr_eval_ref(pr, k, t0, nt, x + t * eta, wt=wt) for t in ts]
+        c = np.polyfit(ts, [r["cost"] for r in rs], 4)
+        dcost = c[-2]
+        assert abs(dcost - (-2.0 * np.dot(r0["vec"], eta))) <= 1e-12 * r0["cost_scale"]
+        V = np.array([r["vec"] for r in rs])
+        dvec = np.polyfit(ts, V, 4)[-2]
+        h = rtr_eval_ref(pr, k, t0, nt, x, eta=eta, wt=wt)
+        _assert_vec(dvec, h["vec"], h["vec_scale"], 1e-11)
+        # a real error would be far above the bound
+        assert np.abs(h["vec"]).max() > 1e-3 * h["vec_scale"].max()
 
 
 @needs_oracle

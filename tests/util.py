@@ -66,6 +66,94 @@ def line_model_ref(pr, xk, pk):
     return tuple(_api_layout(v) for v in V)
 
 
+def _jones(vec, N):
+    """8N parameter vector (station s: J[a][m] at 8s + 2(2a+m)) -> [N, 2, 2] complex"""
+    J = np.asarray(vec, dtype=np.float64).reshape(N, 4, 2)
+    return (J[..., 0] + 1j * J[..., 1]).reshape(N, 2, 2)
+
+
+def _chunk_rows(pr, k, t0, nt, y):
+    """hidden data d, coherencies C of cluster k, unflagged mask and stations of the chunk's rows"""
+    r0, r1 = t0 * pr.Nbase, (t0 + nt) * pr.Nbase
+    dd = np.asarray(y, dtype=np.float64)[8 * r0:8 * r1].reshape(-1, 4, 2)
+    d = (dd[..., 0] + 1j * dd[..., 1]).reshape(-1, 2, 2)
+    C = pr.coh.reshape(pr.Nbase1, pr.M, 2, 2)[r0:r1, k]
+    return d, C, pr.flag[r0:r1] == 0, pr.sta1[r0:r1], pr.sta2[r0:r1]
+
+
+def _station_sums(pr, nt, vp, vq):
+    """per-row 2x2 terms of the p and q ends -> per-station sums [N, 2, 2]: summed over the timeslots
+    of each baseline first, then over the baselines of each station"""
+    Nb = pr.Nbase
+    S = np.zeros((pr.N, 2, 2), dtype=vp.dtype)
+    np.add.at(S, pr.sta1[:Nb], vp.reshape(nt, Nb, 2, 2).sum(axis=0))
+    np.add.at(S, pr.sta2[:Nb], vq.reshape(nt, Nb, 2, 2).sum(axis=0))
+    return S
+
+
+def rtr_eval_ref(pr, k, t0, nt, x, eta=None, wt=None, y=None):
+    """plain float64 per-row restatement of the RTR evaluator (rtr_algo.h, evaluator concept) on
+    cluster k, tiles [t0, t0 + nt), hidden data y (default: the problem's data), row weights wt
+    (one per row of the chunk, default 1), flagged rows skipped:
+      cost   sum w |d - Gp C Gq^H|^2
+      vec    station sums of w res Gq C^H (at p) and w res^H Gp C (at q); with eta their derivative
+             along eta: w (res Eq - res1 Gq) C^H and w (res^H Ep - res1^H Gp) C, res1 = Gp C Eq^H + Ep C Gq^H
+      counts unflagged rows per station
+    Each value comes with a magnitude companion, the same sums over absolute values with res taken as
+    |d| + |Gp||C||Gq|^T (the tensor form of the kernels subtracts those two): cost_scale
+    sum w (|d|^2 + (|Gp||C||Gq|^T)^2), vec_scale [8N].  Vectors in the parameter layout."""
+    N = pr.N
+    d, C, ok, p, q = _chunk_rows(pr, k, t0, nt, pr.x if y is None else y)
+    w = ok * (1.0 if wt is None else np.asarray(wt, dtype=np.float64))
+    H = lambda A: np.conj(np.swapaxes(A, -1, -2))
+    T = lambda A: np.swapaxes(A, -1, -2)
+    A = np.abs
+    G = _jones(x, N)
+    Gp, Gq = G[p], G[q]
+    V = Gp @ C @ H(Gq)
+    Va = A(Gp) @ A(C) @ T(A(Gq))
+    res = d - V
+    ra = A(d) + Va
+    wr = w[:, None, None]
+    cost = float(np.sum(w * np.sum(np.abs(res) ** 2, axis=(1, 2))))
+    cost_scale = float(np.sum(w * np.sum(np.abs(d) ** 2 + Va ** 2, axis=(1, 2))))
+    if eta is None:
+        vp = wr * (res @ Gq @ H(C))
+        vq = wr * (H(res) @ Gp @ C)
+        sp = wr * (ra @ A(Gq) @ T(A(C)))
+        sq = wr * (T(ra) @ A(Gp) @ A(C))
+    else:
+        E = _jones(eta, N)
+        Ep, Eq = E[p], E[q]
+        res1 = Gp @ C @ H(Eq) + Ep @ C @ H(Gq)
+        r1a = A(Gp) @ A(C) @ T(A(Eq)) + A(Ep) @ A(C) @ T(A(Gq))
+        vp = wr * ((res @ Eq - res1 @ Gq) @ H(C))
+        vq = wr * ((H(res) @ Ep - H(res1) @ Gp) @ C)
+        sp = wr * ((ra @ A(Eq) + r1a @ A(Gq)) @ T(A(C)))
+        sq = wr * ((T(ra) @ A(Ep) + T(r1a) @ A(Gp)) @ A(C))
+    S = _station_sums(pr, nt, vp, vq)
+    Sa = _station_sums(pr, nt, sp, sq)
+    vec = np.stack([S.real, S.imag], axis=-1).reshape(-1)
+    vec_scale = np.stack([Sa, Sa], axis=-1).reshape(-1)
+    counts = (np.bincount(p, weights=ok.astype(float), minlength=N)
+              + np.bincount(q, weights=ok.astype(float), minlength=N))
+    return dict(cost=cost, cost_scale=cost_scale, vec=vec, vec_scale=vec_scale, counts=counts)
+
+
+def rtr_weights_ref(pr, k, t0, nt, x, nu, y=None):
+    """Student's-t row weights (nu+2)/(nu + max_c |res_c|^2) at x on the chunk's unflagged rows (0 on
+    flagged ones) and sum(log w - w) over the unflagged rows divided by ALL rows of the chunk.
+    returns (slw, w, slw_scale), slw_scale the same mean over |log w| + w"""
+    d, C, ok, p, q = _chunk_rows(pr, k, t0, nt, pr.x if y is None else y)
+    G = _jones(x, pr.N)
+    res = d - G[p] @ C @ np.conj(np.swapaxes(G[q], -1, -2))
+    e2 = np.max((np.abs(res) ** 2).reshape(-1, 4), axis=1)
+    w = np.where(ok, (nu + 2.0) / (nu + e2), 0.0)
+    lw = np.where(ok, np.log(np.where(ok, w, 1.0)), 0.0)
+    n = len(ok)
+    return float(np.sum(lw - w)) / n, w, float(np.sum(np.abs(lw) + w)) / n
+
+
 def big_cluster_sky(seed=7, sizes=(1, 95, 96, 97, 192, 200, 0)):
     """clusters of the given sizes (0: empty), half the sources Gaussian, spread over a few
     degrees, fluxes with a spectral index"""
