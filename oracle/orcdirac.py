@@ -59,6 +59,8 @@ class Oracle:
         L.orc_grad.argtypes = [pp, dp, dp, dp, i, d]
         L.orc_normal_eq.restype = d
         L.orc_normal_eq.argtypes = [pp, i, i, i, dp, dp, dp, dp, dp]
+        L.orc_normal_eq_os.restype = None
+        L.orc_normal_eq_os.argtypes = [pp, i, i, i, dp, dp, dp, i, dp, dp]
         L.orc_lm_chunk.argtypes = [pp, i, i, i, dp, dp, i, dp, i, i, dp]
         L.orc_rlm_chunk.argtypes = [pp, i, i, i, dp, dp, i, i, i, d, d, dp, dp]
         L.orc_update_w_and_nu.restype = d
@@ -120,6 +122,13 @@ class Oracle:
         self.L.orc_predict_cluster(C.byref(self.P), k, _d(pp), _d(out))
         return out
 
+    def predict_chunk(self, k, t0, ntiles, pblk):
+        """model of cluster k with one parameter block over tiles [t0, t0 + ntiles)"""
+        out = np.zeros(8 * ntiles * self.pr.Nbase)
+        self.L.orc_predict_chunk(C.byref(self.P), k, t0, ntiles,
+                                 _d(np.ascontiguousarray(pblk, dtype=np.float64)), _d(out))
+        return out
+
     def cost(self, pp, x, robust=False, nu=2.0):
         return self.L.orc_cost(C.byref(self.P), _d(pp), _d(x), int(robust), nu)
 
@@ -143,6 +152,19 @@ class Oracle:
         c = self.L.orc_normal_eq(C.byref(self.P), k, t0, ntiles, _d(pblk), _d(xd),
                                  _d(wt) if wt is not None else None, _d(JTJ.reshape(-1)), _d(JTe))
         return c, JTJ, JTe
+
+    def normal_eq_os(self, k, t0, ntiles, pblk, e_full, wt, l):
+        """J^T J, J^T e of ordered subset l with the reference's pairing (orc_normal_eq_os): e_full is
+        the chunk's residual as the LM holds it (weighted by wt), wt its sqrt-weights or None"""
+        n8 = 8 * self.pr.N
+        JTJ = np.zeros((n8, n8))
+        JTe = np.zeros(n8)
+        pblk = np.ascontiguousarray(pblk, dtype=np.float64)
+        e_full = np.ascontiguousarray(e_full, dtype=np.float64)
+        wt = None if wt is None else np.ascontiguousarray(wt, dtype=np.float64)
+        self.L.orc_normal_eq_os(C.byref(self.P), k, t0, ntiles, _d(pblk), _d(e_full),
+                                _d(wt) if wt is not None else None, l, _d(JTJ.reshape(-1)), _d(JTe))
+        return JTJ, JTe
 
     def lm_chunk(self, k, t0, ntiles, pblk, xd, itmax, opts=(1e-3, 1e-15, 1e-15, 1e-20, -1e-6),
                  linsolv=0, os_=False):

@@ -588,6 +588,98 @@ struct LmOut {
   bool res_in_dbuf;
 };
 
+// Subsets of the ordered-subsets LM of a chunk of `ntiles` tiles (clmfit.c:1313-1356): Nsubsets
+// pieces of Ntper tiles.  They coincide with the pieces of the data only when the tile count is a
+// multiple of the subset count.
+struct OsLayout {
+  int Nsubsets, Ntper;
+  bool misaligned;
+};
+static OsLayout os_layout(int ntiles) {
+  OsLayout o;
+  o.Nsubsets = ntiles < 10 ? ntiles : 10;
+  o.Ntper = o.Nsubsets > 0 ? (ntiles + o.Nsubsets - 1) / o.Nsubsets : ntiles;
+  o.misaligned = o.Nsubsets > 0 && (ntiles % o.Nsubsets) != 0 && !db_opt(DB_OPT_OS_CONSISTENT);
+  return o;
+}
+
+// what os_subset_system ran: the subset's tiles [s0, s1) and, on the misaligned branch, the number
+// of Jacobian rows nJ that are paired with data
+struct OsPath {
+  bool misaligned;
+  int s0, s1;
+  long long nJ;
+};
+
+// J^T e (w.JTe) and J^T J (w.JTJ0) of ordered subset l of chunk ck of cluster k, tiles [t0, t1), at
+// pblk_dev; the hidden data are in w.dbuf, wt are the sqrt-weights (robust LM) or null.
+static OsPath os_subset_system(dirac_b200_problem *pr, int k, int t0, int t1, int l,
+                               const double *pblk_dev, const double2 *wt) {
+  DevProblem &d = pr->d;
+  LMWork &w = pr->lm;
+  const int ntiles = t1 - t0;
+  const OsLayout L = os_layout(ntiles);
+  const int Ntper = L.Ntper;
+  OsPath path;
+  path.misaligned = L.misaligned;
+  path.nJ = 0;
+  int s0 = t0 + l * Ntper;
+  int s1 = (l * Ntper + Ntper < ntiles) ? s0 + Ntper : t1;
+  if (s0 > t1) s0 = t1;
+  if (!L.misaligned) {
+    // J^T e restricted to the subset; e is the current (weighted) residual d - f(p)
+    db_cluster_pass(pr, k, pblk_dev, w.dbuf, nullptr, 1, 0, w.JTe, 2, s0, s1, wt);
+    if (wt) {
+      weighted_jtj(pr, k, s0, s1, pblk_dev, wt, w.JTJ0);
+    } else {
+      gram(pr, k, s0, s1, 1, w.Tsub);
+      assemble(pr, w.Tsub, pblk_dev, w.JTJ0);
+    }
+  } else {
+    // The reference pairs row i of the subset's Jacobian with the residual (and weight) of data
+    // index edI[l] + i, Npersubset = ceil(n/Nsubsets) apart, while the subset's tiles are
+    // Ntpersubset = ceil(ntiles/Nsubsets) apart (clmfit.c:1313-1356,1400; robustlm.c:2835-2935):
+    // when ntiles is not a multiple of Nsubsets that is another tile, baseline and component, and
+    // the Jacobian is cut (or zero padded) to Nos[l] rows.  Reproduced literally: the residual of
+    // the whole chunk at p, gathered with the reference's offset into the subset's rows, enters the
+    // J^T e pass as a given vector; the cut and the weights enter as per-component sqrt-weights.
+    const long long nn = 8ll * ntiles * d.Nbase;
+    const long long Nper = (nn + L.Nsubsets - 1) / L.Nsubsets;
+    const long long kl = (long long)l * Nper;
+    const int tl = l * Ntper;
+    long long Nos;
+    int tileI;
+    if (tl + Ntper < ntiles) {
+      Nos = Nper;
+      tileI = Ntper;
+    } else {
+      Nos = nn - kl;
+      tileI = ntiles - tl;
+    }
+    long long nJ = tileI > 0 ? 8ll * d.Nbase * tileI : 0;
+    if (Nos < nJ) nJ = Nos;
+    if (nJ < 0) nJ = 0;
+    s0 = t0 + tl;
+    s1 = s0 + (tileI > 0 ? tileI : 0);
+    if (s0 > t1) s0 = s1 = t1;
+    os_init(pr);
+    // residual of the whole chunk at p (unweighted), then the shifted gather
+    db_cluster_pass(pr, k, pblk_dev, w.dbuf, w.ebuf, 1, 1, nullptr, 2, t0, t1, nullptr);
+    if (s1 > s0) {
+      db_launch_os_shift(w.ebuf, wt, w.os_eps, w.os_w, d.R, (long long)s0 * d.Nbase,
+                         (long long)(s1 - s0) * d.Nbase, (long long)t0 * d.Nbase, kl, nJ, d.stream);
+      db_count_launch(1);
+    }
+    db_cluster_pass(pr, k, pblk_dev, w.os_eps, nullptr, 4, 0, w.JTe, 2, s0, s1, w.os_w);
+    // the cut of the Jacobian and the shifted weights are in os_w
+    weighted_jtj(pr, k, s0, s1, pblk_dev, w.os_w, w.JTJ0);
+    path.nJ = nJ;
+  }
+  path.s0 = s0;
+  path.s1 = s1;
+  return path;
+}
+
 static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, double *pblk_dev,
                     const double2 *wt, int itmax, const double *opts, int linsolv, int os,
                     int os_shift, int randomize, bool have_first, double first_cost, int *nu_damp,
@@ -652,13 +744,10 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
   int kiter_adjust = 0;
 
   // ordered subsets (clmfit.c:1313-1356)
-  int Nsubsets = 10;
-  if (ntiles < Nsubsets) Nsubsets = ntiles;
+  const OsLayout osl = os_layout(ntiles);
+  const int Nsubsets = osl.Nsubsets;
   const int max_os_iter = os ? (int)ceil(0.1 * (double)Nsubsets) : 1;
-  const int Ntper = (os && Nsubsets > 0) ? (ntiles + Nsubsets - 1) / Nsubsets : ntiles;
-  // subsets of tiles and of data coincide only when the tile count is a multiple of the subset count
-  const bool os_misaligned = os && Nsubsets > 0 && (ntiles % Nsubsets) != 0 &&
-                             !db_opt(DB_OPT_OS_CONSISTENT);
+  const bool os_misaligned = os && osl.misaligned;
 
   // Gram tensor of this chunk (time-invariant part of the unweighted J^T J), built once
   const int tix = d.h_clus[k].chunk0 + ck;
@@ -692,93 +781,38 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
       }
     }
     for (int ositer = 0; ositer < max_os_iter; ositer++) {
-      int s0 = t0, s1 = t1;
-      if (os) {
-        int l;
-        if (randomize) {
-          l = subI[ositer];
-        } else {
-          l = (os_shift + kiter + ositer) % Nsubsets;
-        }
-        s0 = t0 + l * Ntper;
-        s1 = (l * Ntper + Ntper < ntiles) ? s0 + Ntper : t1;
-        if (s0 > t1) s0 = t1;
-        if (!os_misaligned) {
-          // J^T e restricted to the subset; e is the current (weighted) residual d - f(p)
-          db_cluster_pass(pr, k, pblk_dev, w.dbuf, nullptr, 1, 0, w.JTe, 2, s0, s1, wt);
-        } else {
-          // The reference pairs row i of the subset's Jacobian with the residual (and weight) of data
-          // index edI[l] + i, Npersubset = ceil(n/Nsubsets) apart, while the subset's tiles are
-          // Ntpersubset = ceil(ntiles/Nsubsets) apart (clmfit.c:1313-1356,1400; robustlm.c:2835-2935):
-          // when ntiles is not a multiple of Nsubsets that is another tile, baseline and component, and
-          // the Jacobian is cut (or zero padded) to Nos[l] rows.  Reproduced literally: the residual of
-          // the whole chunk at p, gathered with the reference's offset into the subset's rows, enters the
-          // J^T e pass as a given vector; the cut and the weights enter as per-component sqrt-weights.
-          const long long nn = 8ll * ntiles * d.Nbase;
-          const long long Nper = (nn + Nsubsets - 1) / Nsubsets;
-          const long long kl = (long long)l * Nper;
-          const int tl = l * Ntper;
-          long long Nos;
-          int tileI;
-          if (tl + Ntper < ntiles) {
-            Nos = Nper;
-            tileI = Ntper;
-          } else {
-            Nos = nn - kl;
-            tileI = ntiles - tl;
-          }
-          long long nJ = tileI > 0 ? 8ll * d.Nbase * tileI : 0;
-          if (Nos < nJ) nJ = Nos;
-          if (nJ < 0) nJ = 0;
-          s0 = t0 + tl;
-          s1 = s0 + (tileI > 0 ? tileI : 0);
-          if (s0 > t1) s0 = s1 = t1;
-          os_init(pr);
-          // residual of the whole chunk at p (unweighted), then the shifted gather
-          db_cluster_pass(pr, k, pblk_dev, w.dbuf, w.ebuf, 1, 1, nullptr, 2, t0, t1, nullptr);
-          if (s1 > s0) {
-            db_launch_os_shift(w.ebuf, wt, w.os_eps, w.os_w, d.R, (long long)s0 * d.Nbase,
-                               (long long)(s1 - s0) * d.Nbase, (long long)t0 * d.Nbase, kl, nJ, d.stream);
-            db_count_launch(1);
-          }
-          db_cluster_pass(pr, k, pblk_dev, w.os_eps, nullptr, 4, 0, w.JTe, 2, s0, s1, w.os_w);
-        }
-        DB_CHECK(cudaMemcpyAsync(hjte, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToHost,
-                                 d.stream));
-      }
       double mx = 0.0;
       // first iteration of a prefactored cluster: J^T J, mu0 and the factor are already there
       const int slot = (!wt && !os && kiter == 0 && linsolv == 0) ? w.pref_slot[k] : -1;
       const bool prefac = slot >= 0;
       const bool need_mx = (kiter == 0) && !prefac;
       w.jtj0_cur = prefac ? w.JB + (size_t)slot * n * n : nullptr;
-      if (prefac) {
+      if (os) {
+        const int l = randomize ? subI[ositer] : (os_shift + kiter + ositer) % Nsubsets;
+        os_subset_system(pr, k, t0, t1, l, pblk_dev, wt);
+        DB_CHECK(cudaMemcpyAsync(hjte, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToHost,
+                                 d.stream));
+      } else if (prefac) {
         w.pref_slot[k] = -1;  // valid for this visit only
-      } else if (wt || os_misaligned) {
-        // (misaligned ordered subset: the cut of the Jacobian and the shifted weights are in os_w)
-        weighted_jtj(pr, k, s0, s1, pblk_dev, os_misaligned ? w.os_w : wt, w.JTJ0);
-        if (need_mx) {
+      } else if (wt) {
+        weighted_jtj(pr, k, t0, t1, pblk_dev, wt, w.JTJ0);
+      } else if (w.jtj_spec) {
+        // already assembled at this point while the host was deciding on the previous trial
+        w.jtj0_cur = w.jtj_spec;
+        w.jtj_spec = nullptr;
+      } else {
+        assemble(pr, Tfull, pblk_dev, w.JTJ0);
+      }
+      if (need_mx) {
+        if (wt || os_misaligned) {
           db_launch_extract_diag(w.JTJ0, w.JTe_new, n, d.stream);  // JTe_new is free scratch here
           db_count_launch(1);
           DB_CHECK(cudaMemcpyAsync(hsc, w.JTe_new, sizeof(double) * n, cudaMemcpyDeviceToHost,
                                    d.stream));
-        }
-      } else {
-        const double *Tuse = Tfull;
-        if (os) {
-          gram(pr, k, s0, s1, 1, w.Tsub);
-          Tuse = w.Tsub;
-        }
-        if (w.jtj_spec && !os) {
-          // already assembled at this point while the host was deciding on the previous trial
-          w.jtj0_cur = w.jtj_spec;
-          w.jtj_spec = nullptr;
         } else {
-          assemble(pr, Tuse, pblk_dev, w.JTJ0);
-        }
-        if (need_mx)
           DB_CHECK(cudaMemcpyAsync(hH, w.Hst, sizeof(double) * 4 * d.N, cudaMemcpyDeviceToHost,
                                    d.stream));
+        }
       }
       if (need_mx || os) db_stream_sync(d.stream);
       if (need_mx) {
@@ -1138,6 +1172,37 @@ static double pick_nu(double sumq, double nulow, double nuhigh) {
   return nulow + (double)best * deltanu;
 }
 
+// The update between two IRLS rounds of the robust LM on the rows of tiles [t0, t1) (robustlm.c:
+// 2533-2566): e = d - f(pe) unweighted from the hidden data in w.dbuf, lambda = sum |w_old|, w_i =
+// sqrt((nu0+1)/(nu0+e_i^2)) into w.wbuf, sumq = mean |w - log w|, nu by pick_nu, then the weights
+// scaled by lambda / ndata.  Returns the new nu; out3 (optional) gets (lambda, sumq, nu).
+static double irls_update(dirac_b200_problem *pr, int k, int t0, int t1, const double *pe,
+                          double nu0, double nulow, double nuhigh, double *out3) {
+  DevProblem &d = pr->d;
+  LMWork &w = pr->lm;
+  const long long r0 = (long long)t0 * d.Nbase, r1 = (long long)t1 * d.Nbase;
+  const double ndata = 8.0 * (double)(r1 - r0);
+  db_cluster_pass(pr, k, pe, w.dbuf, w.ebuf, 1, 1, nullptr, 2, t0, t1, nullptr);
+  db_launch_sum_abs(w.wbuf, d.R, r0, r1, pr->partials, d.scal + 3, d.counters, d.stream);
+  db_launch_update_weights(w.ebuf, w.wbuf, d.R, r0, r1, nu0, pr->partials, d.scal + 4, d.counters,
+                           d.stream);
+  db_count_launch(2);
+  DB_CHECK(cudaMemcpyAsync(d.h_scal + 3, d.scal + 3, 2 * sizeof(double), cudaMemcpyDeviceToHost,
+                           d.stream));
+  db_stream_sync(d.stream);
+  const double lambda = d.h_scal[3];
+  const double sumq = d.h_scal[4] / ndata;
+  const double nu = pick_nu(sumq, nulow, nuhigh);
+  db_launch_scale_vis(w.wbuf, d.R, r0, r1, lambda / ndata, 0, d.stream);
+  db_count_launch(1);
+  if (out3) {
+    out3[0] = lambda;
+    out3[1] = sumq;
+    out3[2] = nu;
+  }
+  return nu;
+}
+
 // ------------------------------------------------------------------------------------------------
 // robust LM on chunk ck of cluster k (rlevmar / osrlevmar): three IRLS rounds of weighted LM;
 // between rounds w_i = sqrt((nu+1)/(nu+e_i^2)) from the unweighted residual, nu re-estimated,
@@ -1156,7 +1221,6 @@ void db_rlm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
   int t0, t1;
   chunk_range(d, k, ck, &t0, &t1);
   const long long r0 = (long long)t0 * d.Nbase, r1 = (long long)t1 * d.Nbase;
-  const double ndata = 8.0 * (double)(r1 - r0);
   // hidden data d = beta r + f(p_old)
   const double beta = pr->world > 1 ? pr->beta : 1.0;
   if (!hidden_ready) {
@@ -1180,19 +1244,7 @@ void db_rlm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
       // (unit-weight) residual of the LAST evaluated point, which is a rejected trial if the loop
       // stopped right after one (clmfit.c:478); later rounds recompute it at p (robustlm.c:2538)
       const double *pe = (nw == 0 && evaluated) ? w.plast : pblk_dev;
-      db_cluster_pass(pr, k, pe, w.dbuf, w.ebuf, 1, 1, nullptr, 2, t0, t1, nullptr);
-      db_launch_sum_abs(w.wbuf, d.R, r0, r1, pr->partials, d.scal + 3, d.counters, d.stream);
-      db_launch_update_weights(w.ebuf, w.wbuf, d.R, r0, r1, nu_t, pr->partials, d.scal + 4,
-                               d.counters, d.stream);
-      db_count_launch(2);
-      DB_CHECK(cudaMemcpyAsync(d.h_scal + 3, d.scal + 3, 2 * sizeof(double),
-                               cudaMemcpyDeviceToHost, d.stream));
-      db_stream_sync(d.stream);
-      const double lambda = d.h_scal[3];
-      const double sumq = d.h_scal[4] / ndata;
-      nu_t = pick_nu(sumq, nulow, nuhigh);
-      db_launch_scale_vis(w.wbuf, d.R, r0, r1, lambda / ndata, 0, d.stream);
-      db_count_launch(1);
+      nu_t = irls_update(pr, k, t0, t1, pe, nu_t, nulow, nuhigh, nullptr);
     }
   }
   *robust_nu = nu_t;
@@ -1251,6 +1303,83 @@ extern "C" double dirac_b200_normal_eq_weighted(dirac_b200_problem *pr, int clus
     DB_CHECK(cudaMemcpy(JTJ, w.JTJ0, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost));
   DB_CHECK(cudaGetLastError());
   return c;
+}
+
+// ------------------------------------------------------------------------------------------------
+// test hooks (not in the public header): the ordered-subsets system, the IRLS update and the chunk
+// solves of the LM, each through the code the solvers run, on caller-supplied hidden data
+// ------------------------------------------------------------------------------------------------
+// J^T J and J^T e that lm_core forms for subset l of chunk `chunk` of cluster clus at pblk, on hidden
+// data xd with sqrt-weights wt (API layout, full interval) or none.  path = (misaligned, s0, s1, nJ).
+extern "C" void dirac_b200_os_normal_eq(dirac_b200_problem *pr, int clus, int chunk, int l,
+                                        const double *pblk, const double *xd, const double *wt,
+                                        double *JTJ, double *JTe, long long *path) {
+  DevProblem &d = pr->d;
+  db_lm_init(pr);
+  robust_init(pr);
+  LMWork &w = pr->lm;
+  const int n = w.n8;
+  int t0, t1;
+  chunk_range(d, clus, chunk, &t0, &t1);
+  db_upload_vis(pr, xd, w.dbuf);
+  if (wt) db_upload_vis(pr, wt, w.wbuf);
+  DB_CHECK(cudaMemcpyAsync(w.pnew, pblk, sizeof(double) * n, cudaMemcpyHostToDevice, d.stream));
+  const OsPath p = os_subset_system(pr, clus, t0, t1, l, w.pnew, wt ? w.wbuf : nullptr);
+  DB_CHECK(cudaMemcpyAsync(JTe, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToHost, d.stream));
+  DB_CHECK(cudaMemcpyAsync(JTJ, w.JTJ0, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost,
+                           d.stream));
+  db_stream_sync(d.stream);
+  DB_CHECK(cudaGetLastError());
+  path[0] = p.misaligned ? 1 : 0;
+  path[1] = p.s0;
+  path[2] = p.s1;
+  path[3] = p.nJ;
+}
+
+// the update between two IRLS rounds on chunk `chunk` of cluster clus: residual at pblk of the
+// hidden data xd, new weights from wt_inout (API layout, full interval; rows outside the chunk are
+// left as they are) with nu0, nu of [nulow, nuhigh).  out3 = (lambda, sumq, nu).
+extern "C" void dirac_b200_irls_update(dirac_b200_problem *pr, int clus, int chunk,
+                                       const double *pblk, const double *xd, double *wt_inout,
+                                       double nu0, double nulow, double nuhigh, double *out3) {
+  DevProblem &d = pr->d;
+  db_lm_init(pr);
+  robust_init(pr);
+  LMWork &w = pr->lm;
+  int t0, t1;
+  chunk_range(d, clus, chunk, &t0, &t1);
+  db_upload_vis(pr, xd, w.dbuf);
+  db_upload_vis(pr, wt_inout, w.wbuf);
+  DB_CHECK(cudaMemcpyAsync(w.pnew, pblk, sizeof(double) * w.n8, cudaMemcpyHostToDevice, d.stream));
+  irls_update(pr, clus, t0, t1, w.pnew, nu0, nulow, nuhigh, out3);
+  db_download_vis(pr, w.wbuf, wt_inout);
+  DB_CHECK(cudaGetLastError());
+}
+
+// LM (robust == 0: clevmar / oslevmar) or robust LM (rlevmar / osrlevmar) of chunk `chunk` of
+// cluster clus on hidden data xd, from pblk_inout (updated).  opts: the plain LM's (tau, eps1..3) or
+// null; the robust LM uses its own.  nu_inout: the robust LM's nu.  info[10] as the reference's.
+extern "C" void dirac_b200_lm_chunk(dirac_b200_problem *pr, int clus, int chunk, double *pblk_inout,
+                                    const double *xd, int itmax, const double *opts, int linsolv,
+                                    int os, int robust, double nulow, double nuhigh,
+                                    double *nu_inout, double *info) {
+  DevProblem &d = pr->d;
+  db_lm_init(pr);
+  LMWork &w = pr->lm;
+  const int n = w.n8;
+  db_upload_vis(pr, xd, w.dbuf);
+  double *pblk_dev = w.pold;
+  DB_CHECK(cudaMemcpyAsync(pblk_dev, pblk_inout, sizeof(double) * n, cudaMemcpyHostToDevice,
+                           d.stream));
+  if (robust)
+    db_rlm_chunk(pr, clus, chunk, pblk_dev, pr->res, itmax, linsolv, os, 0, nulow, nuhigh, nu_inout,
+                 info, true);
+  else
+    db_lm_chunk(pr, clus, chunk, pblk_dev, pr->res, itmax, opts, linsolv, os, 0, info, true);
+  DB_CHECK(cudaMemcpyAsync(pblk_inout, pblk_dev, sizeof(double) * n, cudaMemcpyDeviceToHost,
+                           d.stream));
+  db_stream_sync(d.stream);
+  DB_CHECK(cudaGetLastError());
 }
 
 // micro-benchmark of the all-cluster predict (cost_mode 1, no output): average device time in us

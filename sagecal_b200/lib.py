@@ -248,6 +248,65 @@ class DeviceProblem:
         return dict(results=res, slw=info[0], nslice=int(info[1]), tslice=int(info[2]),
                     inline=bool(info[3]))
 
+    def os_normal_eq(self, clus, chunk, l, pblk, xd, wt=None):
+        """J^T J and J^T e of ordered subset l as the OS-LM forms them (dirac_b200_os_normal_eq), on
+        hidden data xd with sqrt-weights wt (API layout, full interval) or none.
+        returns (JTJ, JTe, path dict(misaligned, s0, s1, nJ))"""
+        L = self.api.lib
+        L.dirac_b200_os_normal_eq.restype = None
+        L.dirac_b200_os_normal_eq.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, c_double_p,
+                                              c_double_p, c_double_p, c_double_p, c_double_p,
+                                              C.POINTER(C.c_longlong)]
+        n8 = 8 * self.N
+        JTJ = np.zeros((n8, n8))
+        JTe = np.zeros(n8)
+        path = (C.c_longlong * 4)()
+        pblk = np.ascontiguousarray(pblk, dtype=np.float64)
+        xd = np.ascontiguousarray(xd, dtype=np.float64)
+        wt = None if wt is None else np.ascontiguousarray(wt, dtype=np.float64)
+        L.dirac_b200_os_normal_eq(self.h, clus, chunk, l, dptr(pblk), dptr(xd),
+                                  dptr(wt) if wt is not None else None, dptr(JTJ.reshape(-1)),
+                                  dptr(JTe), path)
+        return JTJ, JTe, dict(misaligned=bool(path[0]), s0=int(path[1]), s1=int(path[2]),
+                              nJ=int(path[3]))
+
+    def irls_update(self, clus, chunk, pblk, xd, wt, nu0, nulow=2.0, nuhigh=30.0):
+        """the update between two robust-LM rounds (dirac_b200_irls_update): residual at pblk of the
+        hidden data xd, weights from wt (API layout, full interval) with nu0.
+        returns (new weights [rows outside the chunk as given], lambda, sumq, nu)"""
+        L = self.api.lib
+        L.dirac_b200_irls_update.restype = None
+        L.dirac_b200_irls_update.argtypes = [C.c_void_p, C.c_int, C.c_int, c_double_p, c_double_p,
+                                             c_double_p, C.c_double, C.c_double, C.c_double,
+                                             c_double_p]
+        w = np.array(wt, dtype=np.float64)
+        out3 = np.zeros(3)
+        L.dirac_b200_irls_update(self.h, clus, chunk,
+                                 dptr(np.ascontiguousarray(pblk, dtype=np.float64)),
+                                 dptr(np.ascontiguousarray(xd, dtype=np.float64)), dptr(w), nu0,
+                                 nulow, nuhigh, dptr(out3))
+        return w, out3[0], out3[1], out3[2]
+
+    def lm_chunk(self, clus, chunk, pblk, xd, itmax, opts=None, linsolv=0, os_=False, robust=False,
+                 nulow=2.0, nuhigh=30.0, nu0=2.0):
+        """LM (clevmar / oslevmar) or robust LM (rlevmar / osrlevmar) of one chunk on hidden data xd,
+        through the solvers' own chunk functions (dirac_b200_lm_chunk).
+        returns (pblk, info [10], nu)"""
+        L = self.api.lib
+        L.dirac_b200_lm_chunk.restype = None
+        L.dirac_b200_lm_chunk.argtypes = [C.c_void_p, C.c_int, C.c_int, c_double_p, c_double_p,
+                                          C.c_int, c_double_p, C.c_int, C.c_int, C.c_int, C.c_double,
+                                          C.c_double, C.POINTER(C.c_double), c_double_p]
+        p = np.array(pblk, dtype=np.float64)
+        info = np.zeros(10)
+        nu = C.c_double(nu0)
+        o = None if opts is None else np.ascontiguousarray(opts, dtype=np.float64)
+        L.dirac_b200_lm_chunk(self.h, clus, chunk, dptr(p),
+                              dptr(np.ascontiguousarray(xd, dtype=np.float64)), itmax,
+                              dptr(o) if o is not None else None, linsolv, int(os_), int(robust),
+                              nulow, nuhigh, C.byref(nu), dptr(info))
+        return p, info, nu.value
+
     def normal_eq(self, clus, chunk, pblk, xd):
         n8 = 8 * self.N
         JTJ = np.zeros((n8, n8))

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 import orcdirac
-from util import (big_cluster_sky, line_model_ref, relerr, rtr_eval_ref, rtr_weights_ref,
+from util import (big_cluster_sky, irls_ref, line_model_ref, relerr, rtr_eval_ref, rtr_weights_ref,
                   small_problem, split_cluster)
 
 needs_oracle = pytest.mark.skipif(not orcdirac.available(), reason="oracle/liboracle.so not built")
@@ -99,6 +99,33 @@ def test_rtr_eval_reference_is_the_derivative_of_the_cost(weighted):
         _assert_vec(dvec, h["vec"], h["vec_scale"], 1e-11)
         # a real error would be far above the bound
         assert np.abs(h["vec"]).max() > 1e-3 * h["vec_scale"].max()
+
+
+@needs_oracle
+@pytest.mark.parametrize("data,nu0", [("outliers", 2.0), ("outliers", 7.6), ("clean", 30.0)])
+def test_irls_reference_matches_oracle(data, nu0):
+    """util.irls_ref against orc_update_w_and_nu (pinned to the compiled reference's update_w_and_nu
+    by test_oracle_vs_ref.py): the same nu and weights; with non-unit incoming weights the new ones
+    are scaled by lambda / ndata"""
+    rng = np.random.default_rng(17)
+    e = rng.normal(0, 0.5, 8 * 3000)
+    if data == "outliers":
+        hit = rng.random(e.size) < 0.02
+        e[hit] += rng.normal(0, 5.0, hit.sum())
+    orc = orcdirac.Oracle(small_problem().pr)
+    nu_o, w_o = orc.update_w_and_nu(nu0, e)
+    r = irls_ref(e, np.ones_like(e), nu0)
+    assert r["margin"] > 1e-9
+    assert r["nu"] == nu_o
+    assert r["lam"] == e.size
+    assert relerr(r["w"], w_o) < 1e-15
+    wt_old = rng.uniform(0.2, 1.3, e.size)
+    r2 = irls_ref(e, wt_old, nu0)
+    assert r2["nu"] == nu_o
+    assert abs(r2["lam"] - np.abs(wt_old).sum()) <= 1e-13 * r2["lam"]
+    assert relerr(r2["w"], w_o * (r2["lam"] / e.size)) < 1e-15
+    # clean data sits at the top of the grid, 2 % outliers well below it
+    assert (r["nu"] == 2.0 + 29 * (28.0 / 30)) == (data == "clean")
 
 
 @needs_oracle

@@ -202,6 +202,39 @@ def test_coherencies_and_multifreq(ref):
         assert relerr(xb, xa) < 1e-13
 
 
+@pytest.mark.parametrize("flags", [False, True], ids=["unflagged", "flagged"])
+@pytest.mark.parametrize("T", [3, 10, 12, 15, 25, 33])
+def test_normal_eq_os_matches_the_reference_jacobian(ref, T, flags):
+    """orc_normal_eq_os against the system built literally from the compiled reference's own dense
+    Jacobian and model (ref.lm_jac / ref.lm_func) with the subset pairing of clmfit.c:1313-1413, every
+    subset, unit and non-unit weights.  The dense answers are too large to store: this runs where the
+    reference is built."""
+    from util import os_subset_ref
+    kw = dict(flag_frac=0.3, uvcut_frac=0.03) if flags else dict(uvcut_frac=0.0)
+    b = small_problem(N=8, M=2, tilesz=T, seed=60 + T, **kw)
+    pr = b.pr
+    orc = orcdirac.Oracle(pr)
+    k, n8 = 1, 8 * pr.N
+    pblk = perturbed_jones(pr, seed=T)[n8 * k:n8 * (k + 1)]
+    md = ref.me_data(pr.N, pr.Nbase, T, b.barr, b.sky, pr.coh, clus=k)
+    nn = 8 * T * pr.Nbase
+    J = ref.lm_jac(pblk, md, nn)
+    e = pr.x - ref.lm_func(pblk, md, nn)
+    if np.isnan(J).any():
+        pytest.skip("the reference's Jacobian is stored as a sample only")
+    assert relerr(e, pr.x - orc.predict_chunk(k, 0, T, pblk)) < 1e-14
+    wt = np.random.default_rng(T).uniform(0.2, 1.5, nn)
+    for w in (None, wt):
+        for l in range(min(10, T)):
+            JTJ, JTe, (kl, Nos, tl, tileI) = os_subset_ref(J, e, w, T, pr.Nbase, l)
+            oJTJ, oJTe = orc.normal_eq_os(k, 0, T, pblk, e if w is None else w * e, w, l)
+            if tileI <= 0 or Nos <= 0:
+                assert not oJTJ.any() and not oJTe.any()
+                continue
+            assert relerr(oJTJ, JTJ) < 1e-12, (l, relerr(oJTJ, JTJ))
+            assert relerr(oJTe, JTe) < 1e-12, (l, relerr(oJTe, JTe))
+
+
 @pytest.mark.parametrize("T", [12, 15, 25, 33])
 @pytest.mark.parametrize("robust", [False, True], ids=["oslm", "osrlm"])
 def test_os_subsets_with_the_reference_pairing(ref, T, robust):

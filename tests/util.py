@@ -154,6 +154,70 @@ def rtr_weights_ref(pr, k, t0, nt, x, nu, y=None):
     return float(np.sum(lw - w)) / n, w, float(np.sum(np.abs(lw) + w)) / n
 
 
+def _digamma(x):
+    """the reference's digamma series (updatenu.c:36-49)"""
+    r = 0.0
+    while x < 7.0:
+        r -= 1.0 / x
+        x += 1.0
+    x -= 0.5
+    xx = 1.0 / x
+    xx2 = xx * xx
+    xx4 = xx2 * xx2
+    return (r + np.log(x) + (1. / 24.) * xx2 - (7.0 / 960.0) * xx4 + (31.0 / 8064.0) * xx4 * xx2
+            - (127.0 / 30720.0) * xx4 * xx4)
+
+
+def irls_ref(e, wt_old, nu0, nulow=2.0, nuhigh=30.0):
+    """the update between two IRLS rounds of the robust LM, restated (robustlm.c:2533-2566,
+    updatenu.c:86-104,137-262) for the chunk's residual e and its sqrt-weights wt_old (flat, 8 values
+    per row): w = (nu0+1)/(nu0+e^2), q = |w - log w|, lambda = sum |wt_old|, sumq = sum q / ndata,
+    nu = the point of the 30-point grid on [nulow, nuhigh) with the smallest
+    |psi((nu+1)/2) - ln((nu+1)/2) - psi(nu/2) + ln(nu/2) - sumq + 1| (first one on a tie), new weights
+    sqrt(w) lambda / ndata.  Sums in long double.  returns dict(w, lam, sumq, nu, margin: runner-up
+    |value| minus the best one)"""
+    e = np.asarray(e, dtype=np.float64)
+    n = e.size
+    w = (nu0 + 1.0) / (nu0 + e * e)
+    lam = lsum(np.abs(wt_old))
+    sumq = lsum(np.abs(w - np.log(w))) / n
+    deltanu = (nuhigh - nulow) / 30.0
+    nus = [nulow + float(ci) * deltanu for ci in range(30)]
+    qs = np.array([abs(_digamma(t * 0.5 + 0.5) - np.log((t + 1.0) * 0.5) - _digamma(t * 0.5)
+                       + np.log(t * 0.5) - sumq + 1.0) for t in nus])
+    best = int(np.argmin(qs))
+    return dict(w=np.sqrt(w) * (lam / n), lam=lam, sumq=sumq, nu=nus[best],
+                margin=float(np.sort(qs)[1] - qs[best]))
+
+
+def os_subset_ref(J, e, wt, ntiles, Nbase, l):
+    """the system of ordered subset l as the reference's oslevmar / osrlevmar form it
+    (clmfit.c:1313-1413, robustlm.c:2835-2935), built literally from the chunk's dense Jacobian J
+    [8 ntiles Nbase, 8N], unweighted residual e and sqrt-weights wt (None: 1): the rows of the subset's
+    Ntper tiles, cut or zero padded to Nos rows, paired with e[kl:kl+Nos] and wt[kl:kl+Nos].
+    returns (JTJ, JTe, (kl, Nos, tl, tileI))"""
+    n = 8 * ntiles * Nbase
+    ns = min(10, ntiles)
+    Nper = (n + ns - 1) // ns
+    Ntper = (ntiles + ns - 1) // ns
+    kl, tl = l * Nper, l * Ntper
+    if tl + Ntper < ntiles:
+        Nos, tileI = Nper, Ntper
+    else:
+        Nos, tileI = n - kl, ntiles - tl
+    m8 = J.shape[1]
+    Jos = np.zeros((max(Nos, 0), m8))
+    if tileI > 0 and Nos > 0:
+        Jl = J[8 * Nbase * tl:8 * Nbase * (tl + tileI)]
+        m = min(Nos, len(Jl))
+        Jos[:m] = Jl[:m]
+    w = np.ones(n) if wt is None else np.asarray(wt, dtype=np.float64)
+    ww = w[kl:kl + max(Nos, 0)]
+    ew = (w * e)[kl:kl + max(Nos, 0)]
+    Jw = Jos * ww[:, None]
+    return Jw.T @ Jw, Jw.T @ ew, (kl, Nos, tl, tileI)
+
+
 def big_cluster_sky(seed=7, sizes=(1, 95, 96, 97, 192, 200, 0)):
     """clusters of the given sizes (0: empty), half the sources Gaussian, spread over a few
     degrees, fluxes with a spectral index"""
