@@ -212,28 +212,9 @@ __device__ __forceinline__ int row_chunk(long long r, long long R, int nchunk) {
 // ------------------------------------------------------------------------------------------------
 // kernel argument blocks
 // ------------------------------------------------------------------------------------------------
-struct PredictArgs {
-  const double2 *coh;        // [M][4][R]
-  const double2 *x;          // [4][R] data
-  const unsigned char *flag; // [R]
-  const double *pp;          // Jones
-  const ClusterDesc *clus;   // [M]
-  const int *chunk_poff;     // [Mt]
-  const TileDesc *tiles;
-  double2 *out;              // [4][R] residual (data - model) or model, may be null
-  double *partials;          // [nblocks]
-  double *cost;              // scalar out
-  unsigned int *counter;
-  long long R;
-  int N, Nbase, tilesz, M;
-  int out_mode;              // 0 none, 1 residual x - V, 2 model V
-  int cost_mode;             // 0 none, 1 sum e^2, 2 sum log(1 + e^2/nu)
-  double inv_nu;
-};
-
 struct GradArgs {
   const double2 *coh;        // [M][4][R]
-  const double2 *res;        // [4][R] residual e = data - model (written by k_predict_full)
+  const double2 *res;        // [4][R] residual e = data - model (written by k_stream_all<0>)
   const unsigned char *flag;
   const double *pp;
   const ClusterDesc *clus;
@@ -320,22 +301,6 @@ struct StreamAllArgs {
                              // launches shift the base pointers; hybrid chunk maps need the row)
 };
 
-// line model of the LBFGS line search: e(alpha) = E0 - alpha E1 - alpha^2 E2 (kernels_line.cu)
-struct LineSetupArgs {
-  const double2 *coh;        // [M][4][R]
-  const double2 *x;          // [4][R] data
-  const unsigned char *flag;
-  const double *xk;          // Jones at the line origin (device, 8*N*Mt)
-  const double *pk;          // search direction (device, 8*N*Mt)
-  const ClusterDesc *clus;
-  const int *chunk_poff;
-  const TileDesc *tiles;
-  double2 *E0, *E1, *E2;     // [4][R] each
-  long long R;
-  int N, Nbase, tilesz, M;
-  int partial;               // 1: write the raw sums V0,V1,V2 of the local clusters (sharded run)
-};
-
 struct GramArgs {
   const double2 *coh;        // [M][4][R], cluster of blockIdx.y is k0 + blockIdx.y
   const unsigned char *flag;
@@ -391,9 +356,6 @@ void db_launch_coh_from_planar(const double2 *src, double2 *dst, long long r0, i
                                long long R, cudaStream_t st);
 void db_launch_vis_to_planar(const double2 *src, double2 *dst, long long R, cudaStream_t st);
 void db_launch_vis_from_planar(const double2 *src, double2 *dst, long long R, cudaStream_t st);
-int db_predict_nblocks(int ntile, int tilesz);
-void db_launch_predict_full(const PredictArgs *a, int ntile, cudaStream_t st);
-void db_launch_grad_full(const GradArgs *a, int ntile, cudaStream_t st);
 void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st);
 int db_cluster_pass_nblocks(int ntile, int nt, int tslice);
 void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st);

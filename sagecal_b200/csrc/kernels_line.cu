@@ -7,10 +7,10 @@
 //     (J_p + a D_p) C (J_q + a D_q)^H = V0 + a V1 + a^2 V2 ,
 // so the residual is e(a) = E0 - a E1 - a^2 E2 with
 //     E0 = x - sum_k Jp C Jq^H,  E1 = sum_k (Dp C Jq^H + Jp C Dq^H),  E2 = sum_k Dp C Dq^H .
-// k_line_setup makes ONE pass over the coherencies and leaves E0,E1,E2 (3 x 64 B per row) in HBM/L2;
-// k_line_eval then gives the Gaussian or Student's-t cost at any alpha from those 192 B per row
-// (14.5 MB per vector at C2: L2 resident), and k_line_residual the residual at the accepted step for
-// the gradient pass.  Same arithmetic function of alpha as the reference, 30x less HBM traffic.
+// k_stream_all<1> (kernels_tma.cu) makes ONE pass over the coherencies and leaves E0,E1,E2 (3 x 64 B
+// per row) in HBM/L2; k_line_eval then gives the Gaussian or Student's-t cost at any alpha from
+// those 192 B per row (14.5 MB per vector at C2: L2 resident), and k_line_residual the residual at
+// the accepted step for the gradient pass.  Same arithmetic function of alpha as the reference, 30x less HBM traffic.
 #include "internal.cuh"
 
 __device__ __forceinline__ void grid_reduce_sum_l(double v, double *partials, double *out,
@@ -46,74 +46,6 @@ __device__ __forceinline__ void grid_reduce_sum_l(double v, double *partials, do
       for (int i = 0; i < nw; i++) tot += wsum[i];
       *out = tot;
       *counter = 0;
-    }
-  }
-}
-
-template <int TB>
-__global__ void __launch_bounds__(TILE_THREADS)
-k_line_setup(LineSetupArgs a) {
-  const TileDesc td = a.tiles[blockIdx.x];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int p = td.pb * TILE_P + w;
-  const int q = td.qb * TILE_Q + lane;
-  if (!((q > p) && (q < a.N))) return;
-  const int t0 = blockIdx.y * TB;
-  const long long b = baseline_index(p, q, a.N);
-  double2 V0[TB][4], V1[TB][4], V2[TB][4];
-  long long row[TB];
-#pragma unroll
-  for (int i = 0; i < TB; i++) {
-    const int t = t0 + i;
-    row[i] = (long long)(t < a.tilesz ? t : a.tilesz - 1) * a.Nbase + b;
-#pragma unroll
-    for (int c = 0; c < 4; c++) V0[i][c] = V1[i][c] = V2[i][c] = make_double2(0.0, 0.0);
-  }
-  for (int k = 0; k < a.M; k++) {
-    const ClusterDesc cd = a.clus[k];
-    const double2 *ck = a.coh + (long long)k * 4 * a.R;
-    double2 Jp[4], Jq[4], Dp[4], Dq[4];
-    int cur = -1;
-#pragma unroll
-    for (int i = 0; i < TB; i++) {
-      double2 C[4];
-#pragma unroll
-      for (int c = 0; c < 4; c++) C[c] = ld_stream(ck + (long long)c * a.R + row[i]);
-      const int px = row_chunk(row[i], a.R, cd.nchunk);
-      if (px != cur) {
-        const int off = a.chunk_poff[cd.chunk0 + px];
-        load_jones(a.xk + off, p, Jp);
-        load_jones(a.xk + off, q, Jq);
-        load_jones(a.pk + off, p, Dp);
-        load_jones(a.pk + off, q, Dq);
-        cur = px;
-      }
-      double2 A[4], B[4];
-      mat_ab(Jp, C, A);
-      mat_ab(Dp, C, B);
-      mat_abh_acc(A, Jq, V0[i]);
-      mat_abh_acc(B, Jq, V1[i]);
-      mat_abh_acc(A, Dq, V1[i]);
-      mat_abh_acc(B, Dq, V2[i]);
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < TB; i++) {
-    if (t0 + i < a.tilesz) {
-      const bool fl = a.flag[row[i]] != 0;
-#pragma unroll
-      for (int c = 0; c < 4; c++) {
-        const long long ix = (long long)c * a.R + row[i];
-        const double2 xv = ld_stream(a.x + ix);
-        const double2 z = make_double2(0.0, 0.0);
-        if (a.partial) {
-          st_stream(a.E0 + ix, fl ? z : V0[i][c]);
-        } else {
-          st_stream(a.E0 + ix, fl ? xv : csub(xv, V0[i][c]));
-        }
-        st_stream(a.E1 + ix, fl ? z : V1[i][c]);
-        st_stream(a.E2 + ix, fl ? z : V2[i][c]);
-      }
     }
   }
 }
@@ -201,7 +133,7 @@ k_line_residual(const double2 *__restrict__ E0, const double2 *__restrict__ E1,
   }
 }
 
-// sharded runs: out = x - pm (pm = all-reduced partial models); cost like k_predict_full
+// sharded runs: out = x - pm (pm = all-reduced partial models); cost like k_stream_all<0>
 __global__ void __launch_bounds__(256)
 k_residual_cost(const double2 *__restrict__ x, const double2 *__restrict__ pm,
                 double2 *__restrict__ out, long long n4, int out_mode, int cost_mode, double inv_nu,
@@ -278,11 +210,6 @@ k_cluster_rowmap(const double2 *__restrict__ coh_k, const double2 *__restrict__ 
 }
 
 extern "C" {
-#define LINE_TB 2
-void db_launch_line_setup(const LineSetupArgs *a, int ntile, cudaStream_t st) {
-  dim3 grid(ntile, (a->tilesz + LINE_TB - 1) / LINE_TB);
-  k_line_setup<LINE_TB><<<grid, TILE_THREADS, 0, st>>>(*a);
-}
 #define LINE_GRID 592
 void db_launch_line_eval(const double2 *E0, const double2 *E1, const double2 *E2, long long n4,
                          double alpha, int mode, double inv_nu, double *partials, double *out,

@@ -2,13 +2,10 @@
 // coherencies / visibilities in HBM with 128-bit coalesced loads (a warp = one station p against
 // 32 consecutive stations q, 512 contiguous bytes per polarisation product per timeslot).
 //
-//   k_predict_full   : V = sum_k J_kp C_k J_kq^H over all clusters, residual / cost
-//                      (replaces predict_threadfn_withgain_full, lmfit.c:611-688, plus
-//                       cost_func / robust_cost_func, robust_lbfgs.c:674-726)
-//   k_grad_full      : LBFGS gradient over all clusters from a stored residual
+//   k_grad_tma_split : LBFGS gradient over all clusters from a stored residual
 //                      (replaces cpu_calc_deriv(_robust), robust_lbfgs.c:424-560,155-316, which
 //                       loop per PARAMETER over all rows; here one pass over rows)
-//   k_cluster_pass   : per-cluster E-step pass of the LM solver: model of one cluster, residual,
+//   k_cluster_pass*  : per-cluster E-step pass of the LM solver: model of one cluster, residual,
 //                      cost and J^T e in a single sweep (replaces predict_threadfn_withgain(0),
 //                      lmfit.c:64-124,233-296 + the J^T e dgemv of clmfit.c:315)
 //   k_coh_gram       : per-baseline time sums conj(C) (x) C from which J^T J is assembled without
@@ -128,362 +125,6 @@ __device__ __forceinline__ void grid_reduce_sum(double v, double *partials, doub
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// full predict over all clusters
-// ------------------------------------------------------------------------------------------------
-
-template <int TB>
-__global__ void __launch_bounds__(TILE_THREADS)
-k_predict_full(PredictArgs a) {
-  const TileDesc td = a.tiles[blockIdx.x];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int p = td.pb * TILE_P + w;
-  const int q = td.qb * TILE_Q + lane;
-  const bool valid = (q > p) && (q < a.N);
-  const int t0 = blockIdx.y * TB;
-  double cost = 0.0;
-  if (valid) {
-    const long long b = baseline_index(p, q, a.N);
-    double2 acc[TB][4];
-    bool fl[TB];
-    long long row[TB];
-#pragma unroll
-    for (int i = 0; i < TB; i++) {
-      int t = t0 + i;
-      row[i] = (long long)(t < a.tilesz ? t : a.tilesz - 1) * a.Nbase + b;
-      fl[i] = (t < a.tilesz) ? (a.flag[row[i]] != 0) : true;
-#pragma unroll
-      for (int c = 0; c < 4; c++) acc[i][c] = make_double2(0.0, 0.0);
-    }
-    for (int k = 0; k < a.M; k++) {
-      const ClusterDesc cd = a.clus[k];
-      const double2 *ck = a.coh + (long long)k * 4 * a.R;
-      double2 Jp[4], Jq[4];
-      int cur = -1;
-#pragma unroll
-      for (int i = 0; i < TB; i++) {
-        double2 C[4];
-#pragma unroll
-        for (int c = 0; c < 4; c++) C[c] = ld_stream(ck + (long long)c * a.R + row[i]);
-        int px = row_chunk(row[i], a.R, cd.nchunk);
-        if (px != cur) {
-          const double *pblk = a.pp + a.chunk_poff[cd.chunk0 + px];
-          load_jones(pblk, p, Jp);
-          load_jones(pblk, q, Jq);
-          cur = px;
-        }
-        double2 T1[4];
-        mat_ab(Jp, C, T1);
-        mat_abh_acc(T1, Jq, acc[i]);
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < TB; i++) {
-      if (t0 + i < a.tilesz) {
-#pragma unroll
-        for (int c = 0; c < 4; c++) {
-          double2 m = fl[i] ? make_double2(0.0, 0.0) : acc[i][c];
-          double2 xv = make_double2(0.0, 0.0);
-          if (a.out_mode == 1 || a.cost_mode) xv = ld_stream(a.x + (long long)c * a.R + row[i]);
-          double2 e = csub(xv, m);
-          if (a.out_mode == 1) st_stream(a.out + (long long)c * a.R + row[i], e);
-          if (a.out_mode == 2) st_stream(a.out + (long long)c * a.R + row[i], m);
-          if (a.cost_mode == 1) {
-            cost = fma(e.x, e.x, cost);
-            cost = fma(e.y, e.y, cost);
-          } else if (a.cost_mode == 2) {
-            cost += log(1.0 + e.x * e.x * a.inv_nu);
-            cost += log(1.0 + e.y * e.y * a.inv_nu);
-          }
-        }
-      }
-    }
-  }
-  if (a.cost_mode) grid_reduce_sum(cost, a.partials, a.cost, a.counter);
-}
-
-// ------------------------------------------------------------------------------------------------
-// shared epilogue: reduce per-thread station gradients of a tile and add them to g (8 doubles per
-// station).  Gp belongs to station p (shared by the whole warp), Gq to station q (one per lane,
-// shared by the 8 warps of the CTA).  warp-shuffle reduction for p, smem transpose for q.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tile_reduce_station_grad(const double2 *Gp, const double2 *Gq,
-                                                          double *gblk, int p, int q, int N,
-                                                          bool pvalid, double (*sq)[8][TILE_Q],
-                                                          double scale) {
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // station p: butterfly over the 32 lanes
-  double vp[8];
-#pragma unroll
-  for (int c = 0; c < 4; c++) {
-    vp[2 * c] = warp_sum(Gp[c].x);
-    vp[2 * c + 1] = warp_sum(Gp[c].y);
-  }
-  if (pvalid && lane < 8) {
-    double v = vp[0];
-#pragma unroll
-    for (int c = 1; c < 8; c++) v = (lane == c) ? vp[c] : v;
-    atomicAdd(gblk + 8 * (long long)p + lane, scale * v);
-  }
-  // station q: [warp][component][lane] in smem, warp c sums component c over the 8 warps
-#pragma unroll
-  for (int c = 0; c < 4; c++) {
-    sq[w][2 * c][lane] = Gq[c].x;
-    sq[w][2 * c + 1][lane] = Gq[c].y;
-  }
-  __syncthreads();
-  {
-    double s = 0.0;
-#pragma unroll
-    for (int ww = 0; ww < TILE_P; ww++) s += sq[ww][w][lane];
-    if (q < N && s != 0.0) atomicAdd(gblk + 8 * (long long)q + w, scale * s);
-  }
-  __syncthreads();
-}
-
-// contraction of the time-summed outer product W[i][j][l][m] = sum_t R_ij conj(C_lm) with the Jones
-// matrices:   Gp = R Jq C^H -> Gp_il = sum_{j,m} Jq_jm W[i,j,l,m]
-//             Gq = R^H Jp C -> Gq_jm = sum_{i,l} Jp_il conj(W[i,j,l,m])
-// (the 8 reals of Gp/Gq are d(cost)/d(Re,Im of J_p,il / J_q,jm) up to the factor 2, see
-//  DESIGN.md "closed-form gradient"; cf. the per-parameter E_col products of lmfit.c:436-466)
-__device__ __forceinline__ void contract_W(const double2 *W, const double2 *Jp, const double2 *Jq,
-                                           double2 *Gp, double2 *Gq) {
-#pragma unroll
-  for (int i = 0; i < 2; i++)
-#pragma unroll
-    for (int l = 0; l < 2; l++) {
-      double2 s = make_double2(0.0, 0.0);
-#pragma unroll
-      for (int j = 0; j < 2; j++)
-#pragma unroll
-        for (int m = 0; m < 2; m++) cfma(s, Jq[2 * j + m], W[((i * 2 + j) * 2 + l) * 2 + m]);
-      Gp[2 * i + l] = cadd(Gp[2 * i + l], s);
-    }
-#pragma unroll
-  for (int j = 0; j < 2; j++)
-#pragma unroll
-    for (int m = 0; m < 2; m++) {
-      double2 s = make_double2(0.0, 0.0);
-#pragma unroll
-      for (int i = 0; i < 2; i++)
-#pragma unroll
-        for (int l = 0; l < 2; l++) cfmac(s, Jp[2 * i + l], W[((i * 2 + j) * 2 + l) * 2 + m]);
-      Gq[2 * j + m] = cadd(Gq[2 * j + m], s);
-    }
-}
-
-// W += R (x) conj(C)
-__device__ __forceinline__ void accum_W(double2 *W, const double2 *Rm, const double2 *C) {
-#pragma unroll
-  for (int ij = 0; ij < 4; ij++)
-#pragma unroll
-    for (int lm = 0; lm < 4; lm++) cfmac(W[ij * 4 + lm], Rm[ij], C[lm]);
-}
-
-// ------------------------------------------------------------------------------------------------
-// LBFGS gradient over all clusters
-// ------------------------------------------------------------------------------------------------
-
-template <int TB>
-__global__ void __launch_bounds__(TILE_THREADS)
-k_grad_full(GradArgs a) {
-  __shared__ double sq[TILE_P][8][TILE_Q];
-  const TileDesc td = a.tiles[blockIdx.x];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int p = td.pb * TILE_P + w;
-  const int q = td.qb * TILE_Q + lane;
-  const bool valid = (q > p) && (q < a.N);
-  const int t0 = blockIdx.y * TB;
-  const long long b = valid ? baseline_index(p, q, a.N) : 0;
-  double2 Rm[TB][4];
-  long long row[TB];
-  bool use[TB];
-#pragma unroll
-  for (int i = 0; i < TB; i++) {
-    int t = t0 + i;
-    row[i] = (long long)(t < a.tilesz ? t : a.tilesz - 1) * a.Nbase + b;
-    use[i] = valid && (t < a.tilesz) && (a.flag[row[i]] == 0);
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-      double2 e = make_double2(0.0, 0.0);
-      if (use[i]) {
-        e = ld_stream(a.res + (long long)c * a.R + row[i]);
-        if (a.robust) {
-          e.x = e.x / (a.nu + e.x * e.x);
-          e.y = e.y / (a.nu + e.y * e.y);
-        }
-      }
-      Rm[i][c] = e;
-    }
-  }
-  for (int k = 0; k < a.M; k++) {
-    const ClusterDesc cd = a.clus[k];
-    const double2 *ck = a.coh + (long long)k * 4 * a.R;
-    // gradient chunk of a timeslot: t / ceil(tilesz/nchunk)   (robust_lbfgs.c:464-470)
-    const int tpc = (a.tilesz + cd.nchunk - 1) / cd.nchunk;
-    int i0 = 0;
-    while (i0 < TB) {  // runs of timeslots that share a chunk (one run unless hybrid)
-      const int chunk = (t0 + i0 < a.tilesz ? t0 + i0 : a.tilesz - 1) / tpc;
-      double2 W[16];
-#pragma unroll
-      for (int z = 0; z < 16; z++) W[z] = make_double2(0.0, 0.0);
-      int i1 = i0;
-#pragma unroll
-      for (int i = 0; i < TB; i++) {
-        if (i >= i0 && i == i1) {
-          int t = t0 + i;
-          int ch = (t < a.tilesz ? t : a.tilesz - 1) / tpc;
-          if (ch == chunk) {
-            i1 = i + 1;
-            if (use[i]) {
-              double2 C[4];
-#pragma unroll
-              for (int c = 0; c < 4; c++) C[c] = ld_stream(ck + (long long)c * a.R + row[i]);
-              accum_W(W, Rm[i], C);
-            }
-          }
-        }
-      }
-      double *gblk = a.g + a.chunk_poff[cd.chunk0 + chunk];
-      double2 Jp[4], Jq[4], Gp[4], Gq[4];
-#pragma unroll
-      for (int c = 0; c < 4; c++) {
-        Jp[c] = Jq[c] = Gp[c] = Gq[c] = make_double2(0.0, 0.0);
-      }
-      if (valid) {
-        const double *pblk = a.pp + a.chunk_poff[cd.chunk0 + chunk];
-        load_jones(pblk, p, Jp);
-        load_jones(pblk, q, Jq);
-        contract_W(W, Jp, Jq, Gp, Gq);
-      }
-      tile_reduce_station_grad(Gp, Gq, gblk, p, q, a.N, p < a.N - 1, sq, a.scale);
-      i0 = i1;
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// LBFGS gradient over all clusters, TMA-fed: same tile mapping and reductions as k_grad_full, but the
-// coherencies of the next cluster(s) are already on their way into shared memory (one ring of bulk
-// copies per warp: for a fixed station p the 32 lanes' baselines are one contiguous run of rows)
-// while the current cluster is contracted and reduced.  The register-staged version alternates load
-// and reduce phases with 8 warps per SM and tops out near 1 TB/s.
-// ------------------------------------------------------------------------------------------------
-template <int TB, int NST>
-__global__ void __launch_bounds__(TILE_THREADS)
-k_grad_tma(GradArgs a) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  constexpr int STAGE_ELEMS = TB * 4 * 32;  // double2 per stage
-  double (*sq)[8][TILE_Q] = reinterpret_cast<double (*)[8][TILE_Q]>(smem_raw);
-  double2 *ring = reinterpret_cast<double2 *>(smem_raw + sizeof(double) * TILE_P * 8 * TILE_Q);
-  unsigned long long *bars = reinterpret_cast<unsigned long long *>(ring + (size_t)TILE_P * NST * STAGE_ELEMS);
-  const TileDesc td = a.tiles[blockIdx.x];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int p = td.pb * TILE_P + w;
-  const int q0 = td.qb * TILE_Q;
-  const int q = q0 + lane;
-  const bool valid = (q > p) && (q < a.N);
-  const int t0 = blockIdx.y * TB;
-  const int nrows = min(TB, a.tilesz - t0);
-  // the warp's run of baselines: stations qs .. qs+nv-1 against p
-  const int qs = max(q0, p + 1);
-  const int nv = max(0, min(q0 + TILE_Q, a.N) - qs);
-  const long long b0 = nv > 0 ? baseline_index(p, qs, a.N) : 0;
-  const int el = q - qs;  // slot of this lane inside the run (valid lanes only)
-  const long long b = valid ? b0 + el : 0;
-  double2 *my_stage = ring + (size_t)w * NST * STAGE_ELEMS;
-  unsigned long long *my_bar = bars + w * NST;
-  if (lane == 0) {
-#pragma unroll
-    for (int s = 0; s < NST; s++) mbar_init(&my_bar[s], 1);
-    mbar_fence_init();
-  }
-  __syncwarp();
-  auto issue = [&](int k, int s) {
-    const unsigned row_bytes = (unsigned)nv * 16u;
-    mbar_expect_tx(&my_bar[s], (unsigned)nrows * 4u * row_bytes);
-    const double2 *ck = a.coh + (long long)k * 4 * a.R + (long long)t0 * a.Nbase + b0;
-    double2 *dst = my_stage + (size_t)s * STAGE_ELEMS;
-    for (int i = 0; i < nrows; i++)
-#pragma unroll
-      for (int c = 0; c < 4; c++)
-        bulk_g2s(dst + (i * 4 + c) * 32, ck + (long long)c * a.R + (long long)i * a.Nbase, row_bytes,
-                 &my_bar[s]);
-  };
-  if (lane == 0 && nv > 0) {
-#pragma unroll
-    for (int s = 0; s < NST - 1; s++)
-      if (s < a.M) issue(s, s);
-  }
-
-  double2 Rm[TB][4];
-  bool use[TB];
-#pragma unroll
-  for (int i = 0; i < TB; i++) {
-    const int t = t0 + i;
-    const long long row = (long long)(t < a.tilesz ? t : a.tilesz - 1) * a.Nbase + b;
-    use[i] = valid && (t < a.tilesz) && (a.flag[row] == 0);
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-      double2 e = make_double2(0.0, 0.0);
-      if (use[i]) {
-        e = ld_stream(a.res + (long long)c * a.R + row);
-        if (a.robust) {
-          e.x = e.x / (a.nu + e.x * e.x);
-          e.y = e.y / (a.nu + e.y * e.y);
-        }
-      }
-      Rm[i][c] = e;
-    }
-  }
-  for (int k = 0; k < a.M; k++) {
-    const int s = k % NST;
-    if (lane == 0 && nv > 0 && k + NST - 1 < a.M) issue(k + NST - 1, (k + NST - 1) % NST);
-    const ClusterDesc cd = a.clus[k];
-    // gradient chunk of a timeslot: t / ceil(tilesz/nchunk)   (robust_lbfgs.c:464-470)
-    const int tpc = (a.tilesz + cd.nchunk - 1) / cd.nchunk;
-    if (nv > 0) mbar_wait(&my_bar[s], (unsigned)((k / NST) & 1));
-    const double2 *st = my_stage + (size_t)s * STAGE_ELEMS;
-    int i0 = 0;
-    while (i0 < TB) {  // runs of timeslots that share a chunk (one run unless hybrid)
-      const int chunk = (t0 + i0 < a.tilesz ? t0 + i0 : a.tilesz - 1) / tpc;
-      double2 W[16];
-#pragma unroll
-      for (int z = 0; z < 16; z++) W[z] = make_double2(0.0, 0.0);
-      int i1 = i0;
-#pragma unroll
-      for (int i = 0; i < TB; i++) {
-        if (i >= i0 && i == i1) {
-          const int t = t0 + i;
-          const int ch = (t < a.tilesz ? t : a.tilesz - 1) / tpc;
-          if (ch == chunk) {
-            i1 = i + 1;
-            if (use[i]) {
-              double2 C[4];
-#pragma unroll
-              for (int c = 0; c < 4; c++) C[c] = lds_v2(st + (i * 4 + c) * 32 + el);
-              accum_W(W, Rm[i], C);
-            }
-          }
-        }
-      }
-      double *gblk = a.g + a.chunk_poff[cd.chunk0 + chunk];
-      double2 Jp[4], Jq[4], Gp[4], Gq[4];
-#pragma unroll
-      for (int c = 0; c < 4; c++) Jp[c] = Jq[c] = Gp[c] = Gq[c] = make_double2(0.0, 0.0);
-      if (valid) {
-        const double *pblk = a.pp + a.chunk_poff[cd.chunk0 + chunk];
-        load_jones(pblk, p, Jp);
-        load_jones(pblk, q, Jq);
-        contract_W(W, Jp, Jq, Gp, Gq);
-      }
-      // (two CTA barriers inside: every lane is also done with stage s before it is refilled)
-      tile_reduce_station_grad(Gp, Gq, gblk, p, q, a.N, p < a.N - 1, sq, a.scale);
-      i0 = i1;
-    }
-  }
-}
-
 // sums of four values over the warp with 6 double shuffles instead of 20: halves of the warp trade
 // the values they do not keep.  Lane 8*c (c = 0..3) ends up with the warp sum of v[c].
 __device__ __forceinline__ double warp_reduce4(double v0, double v1, double v2, double v3, int lane) {
@@ -501,10 +142,13 @@ __device__ __forceinline__ double warp_reduce4(double v0, double v1, double v2, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// k_grad_tma with the polarisation split of k_cluster_pass_split: two threads per baseline, thread h
-// owns row h of the residual and the half W[i=h] of the accumulator.  16 warps per CTA share the 8
-// TMA rings (the two warps of a station p consume the same stages; warp h=0 is the producer, the CTA
-// barriers of the per-cluster reduction make a consumed stage reusable).
+// LBFGS gradient over all clusters, TMA-fed.  A CTA is a tile of 8 stations p x 32 stations q; the
+// coherencies of the next cluster(s) are already on their way into shared memory (one ring of bulk
+// copies per station p: its 32 lanes' baselines are one contiguous run of rows) while the current
+// cluster is contracted and reduced.  Polarisation split as in k_cluster_pass_split: two threads
+// per baseline, thread h owns row h of the residual and the half W[i=h] of the accumulator.  16
+// warps per CTA share the 8 rings (the two warps of a station p consume the same stages; warp h=0
+// is the producer, the CTA barriers of the per-cluster reduction make a consumed stage reusable).
 // threadIdx.x = h*256 + w*32 + lane.
 // ------------------------------------------------------------------------------------------------
 template <int TB, int NST>
@@ -681,11 +325,9 @@ k_grad_tma_split(GradArgs a) {
 // per-cluster E-step pass (LM): one cluster, one hybrid chunk, timeslots [t_begin, t_end)
 // ------------------------------------------------------------------------------------------------
 
-// GRAD = false (ADD / SUB passes, ordered-subset trials): no W accumulator, about half the registers
-template <bool GRAD>
+// passes without J^T e (ADD / SUB, cost-only trials) that the linear-mapped kernel does not take
 __global__ void __launch_bounds__(TILE_THREADS)
 k_cluster_pass(ClusterPassArgs a) {
-  __shared__ double sq[GRAD ? TILE_P : 1][8][TILE_Q];
   const TileDesc td = a.tiles[blockIdx.x];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int p = td.pb * TILE_P + w;
@@ -694,16 +336,14 @@ k_cluster_pass(ClusterPassArgs a) {
   const int ts = a.t_begin + blockIdx.y * a.tslice;
   const int te = min(ts + a.tslice, a.t_end);
   double cost = 0.0;
-  double2 Jp[4], Jq[4], W[GRAD ? 16 : 1];
-#pragma unroll
-  for (int z = 0; z < (GRAD ? 16 : 1); z++) W[z] = make_double2(0.0, 0.0);
+  double2 Jp[4], Jq[4];
 #pragma unroll
   for (int c = 0; c < 4; c++) Jp[c] = Jq[c] = make_double2(0.0, 0.0);
   if (valid) {
     load_jones(a.pblk, p, Jp);
     load_jones(a.pblk, q, Jq);
     double2 Jpo[4], Jqo[4];
-    const bool recover = (!GRAD) && a.mode == 3 && a.pblk_old != nullptr;
+    const bool recover = a.mode == 3 && a.pblk_old != nullptr;
     const double gamma = recover ? (1.0 - a.beta) / a.beta : 0.0;
     if (recover) {
       load_jones(a.pblk_old, p, Jpo);
@@ -768,7 +408,8 @@ k_cluster_pass(ClusterPassArgs a) {
       }
       if (a.mode <= 1) {
         if (a.wt) {
-          // robust LM: e <- wt.e for the cost, J^T (wt.(wt.e)) for the gradient
+          // robust LM: the cost is ||wt.e||^2.  e <- wt.(wt.e) feeds nothing here, but without that
+          // store the compiler allocates 172 registers instead of 168
 #pragma unroll
           for (int c = 0; c < 4; c++) {
             const double2 wv = ld_stream(a.wt + (long long)c * a.R + row);
@@ -784,18 +425,8 @@ k_cluster_pass(ClusterPassArgs a) {
             cost = fma(e[c].y, e[c].y, cost);
           }
         }
-        if constexpr (GRAD) {
-          if (!fl) accum_W(W, e, C);
-        }
       }
     }
-  }
-  if constexpr (GRAD) {
-    double2 Gp[4], Gq[4];
-#pragma unroll
-    for (int c = 0; c < 4; c++) Gp[c] = Gq[c] = make_double2(0.0, 0.0);
-    if (valid) contract_W(W, Jp, Jq, Gp, Gq);
-    tile_reduce_station_grad(Gp, Gq, a.jte, p, q, a.N, p < a.N - 1, sq, 1.0);
   }
   if (a.mode <= 1) grid_reduce_sum(cost, a.partials, a.cost, a.counter);
 }
@@ -1241,8 +872,9 @@ k_coh_gram(GramArgs a) {
 // ------------------------------------------------------------------------------------------------
 // host-side launchers
 // ------------------------------------------------------------------------------------------------
-template <int TB, int NST>
-static void launch_grad_tma_split(const GradArgs *a, int ntile, cudaStream_t st) {
+// (declared extern "C" in internal.cuh)
+void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st) {
+  constexpr int TB = 4, NST = 2;
   const size_t smem = sizeof(double) * 2 * TILE_P * 8 * TILE_Q +
                       (size_t)TILE_P * NST * TB * 4 * 32 * sizeof(double2) + TILE_P * NST * 8;
   static bool configured = false;
@@ -1254,19 +886,43 @@ static void launch_grad_tma_split(const GradArgs *a, int ntile, cudaStream_t st)
   dim3 grid(ntile, (a->tilesz + TB - 1) / TB);
   k_grad_tma_split<TB, NST><<<grid, 2 * TILE_THREADS, smem, st>>>(*a);
 }
-template <int TB, int NST>
-static void launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st) {
-  const size_t smem = sizeof(double) * TILE_P * 8 * TILE_Q +
-                      (size_t)TILE_P * NST * TB * 4 * 32 * sizeof(double2) + TILE_P * NST * 8;
+
+// the linear-mapped kernel keeps 8N station sums in shared memory next to its ring and one arrival
+// counter per 256-baseline group: arrays too large for either take the tile kernels
+static bool cluster_pass_lin_fits(int N, int Nbase) {
+  return (size_t)5 * 8 * 256 * sizeof(double2) + sizeof(double) * ((8 * N + 1) & ~1) + 40 <=
+             (size_t)200 * 1024 && (Nbase + 255) / 256 <= 1024;
+}
+
+// linear mapping: 256 baselines per CTA, time sliced to about one CTA per SM (<= 32 rows)
+template <bool GRAD>
+static void launch_cluster_pass_lin(const ClusterPassArgs *a, cudaStream_t st) {
+  constexpr int NST = 5;
+  const int nt = a->t_end - a->t_begin;
+  const int nbg = (a->Nbase + 255) / 256;
+  int nsl = (db_sm_count() + nbg - 1) / nbg;
+  if (nsl > nt) nsl = nt;
+  ClusterPassArgs b = *a;
+  b.tslice = (nt + nsl - 1) / nsl;
+  // test hook: rows per CTA forced (drives the multi-row ring on small problems); with J^T e, only
+  // as long as the slices still fit the per-CTA partial buffer
+  const int forced = db_opt(DB_OPT_CP_ROWS);
+  if (forced > 0 && (!GRAD || (nt + forced - 1) / forced <= db_cp_max_slices(a->Nbase, nt)))
+    b.tslice = forced;
+  if (b.tslice > nt) b.tslice = nt;
+  if (b.tslice > 32) b.tslice = 32;
+  const size_t smem = (size_t)NST * 8 * 256 * sizeof(double2) +
+                      sizeof(double) * ((8 * a->N + 1) & ~1) + NST * 8;
   static bool configured = false;
   if (!configured) {
-    DB_CHECK(cudaFuncSetAttribute(k_grad_tma<TB, NST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)smem));
+    DB_CHECK(cudaFuncSetAttribute(k_cluster_pass_lin<NST, GRAD>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     configured = true;
   }
-  dim3 grid(ntile, (a->tilesz + TB - 1) / TB);
-  k_grad_tma<TB, NST><<<grid, TILE_THREADS, smem, st>>>(*a);
+  dim3 grid(nbg, (nt + b.tslice - 1) / b.tslice);
+  k_cluster_pass_lin<NST, GRAD><<<grid, 512, smem, st>>>(b);
 }
+
 extern "C" {
 
 void db_launch_coh_to_planar(const double2 *src, double2 *dst, long long r0, int nr, int M,
@@ -1288,59 +944,8 @@ void db_launch_vis_from_planar(const double2 *src, double2 *dst, long long R, cu
   k_vis_from_planar<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(src, dst, R);
 }
 
-#define PREDICT_TB 4
-int db_predict_nblocks(int ntile, int tilesz) { return ntile * ((tilesz + PREDICT_TB - 1) / PREDICT_TB); }
-void db_launch_predict_full(const PredictArgs *a, int ntile, cudaStream_t st) {
-  dim3 grid(ntile, (a->tilesz + PREDICT_TB - 1) / PREDICT_TB);
-  k_predict_full<PREDICT_TB><<<grid, TILE_THREADS, 0, st>>>(*a);
-}
-void db_launch_grad_full(const GradArgs *a, int ntile, cudaStream_t st) {
-  dim3 grid(ntile, (a->tilesz + PREDICT_TB - 1) / PREDICT_TB);
-  k_grad_full<PREDICT_TB><<<grid, TILE_THREADS, 0, st>>>(*a);
-}
-void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st) {
-  static int cfg = -1;
-  static const bool unsplit = getenv("DIRAC_B200_CP_UNSPLIT") != nullptr;
-  if (!unsplit) {
-    static int scfg = -1;
-    if (scfg < 0) {
-      const char *e = getenv("DIRAC_B200_GRADS_CFG");
-      scfg = e ? atoi(e) : 0;
-    }
-    switch (scfg) {
-      case 1: launch_grad_tma_split<2, 2>(a, ntile, st); return;
-      case 2: launch_grad_tma_split<2, 3>(a, ntile, st); return;
-      case 3: launch_grad_tma_split<4, 3>(a, ntile, st); return;
-      case 4: launch_grad_tma_split<8, 2>(a, ntile, st); return;
-      case 5: launch_grad_tma_split<1, 4>(a, ntile, st); return;
-      default: launch_grad_tma_split<4, 2>(a, ntile, st); return;
-    }
-  }
-  if (cfg < 0) {
-    const char *e = getenv("DIRAC_B200_GRAD_CFG");
-    cfg = e ? atoi(e) : 0;
-  }
-  switch (cfg) {
-    case 1: launch_grad_tma<2, 3>(a, ntile, st); return;
-    case 2: launch_grad_tma<2, 2>(a, ntile, st); return;
-    case 3: launch_grad_tma<4, 3>(a, ntile, st); return;
-    case 4: launch_grad_tma<3, 2>(a, ntile, st); return;
-    default: launch_grad_tma<4, 2>(a, ntile, st); return;
-  }
-}
 int db_cluster_pass_nblocks(int ntile, int nt, int tslice) { return ntile * ((nt + tslice - 1) / tslice); }
-// the linear-mapped kernel keeps 8N station sums in shared memory next to its ring and one arrival
-// counter per 256-baseline group: arrays too large for either take the tile kernels
-static bool cluster_pass_lin_fits(int N, int Nbase) {
-  return (size_t)5 * 8 * 256 * sizeof(double2) + sizeof(double) * ((8 * N + 1) & ~1) + 40 <=
-             (size_t)200 * 1024 && (Nbase + 255) / 256 <= 1024;
-}
-int db_cluster_pass_forms_hidden(int N, int Nbase) {
-  static const bool tiles = getenv("DIRAC_B200_NO_TMA") != nullptr ||
-                            getenv("DIRAC_B200_CP_UNSPLIT") != nullptr ||
-                            getenv("DIRAC_B200_ADDSUB_TILE") != nullptr;
-  return !tiles && cluster_pass_lin_fits(N, Nbase);
-}
+int db_cluster_pass_forms_hidden(int N, int Nbase) { return cluster_pass_lin_fits(N, Nbase); }
 void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st) {
   int nt = a->t_end - a->t_begin;
   dim3 grid(ntile, (nt + a->tslice - 1) / a->tslice);
@@ -1349,74 +954,16 @@ void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st
                     "kernels run (%s:%d)\n", __FILE__, __LINE__);
     exit(1);
   }
-  static const bool no_tma_any = getenv("DIRAC_B200_NO_TMA") != nullptr;
-  const bool lin_ok = cluster_pass_lin_fits(a->N, a->Nbase);
-  if (!(a->jte != nullptr && a->mode <= 1) && !a->wt && !a->in2 && !no_tma_any && lin_ok &&
-      !getenv("DIRAC_B200_ADDSUB_TILE")) {
-    // ADD / SUB / cost-only pass in the linear mapping: the same CTA-wide TMA ring as the gradient
-    // pass, without the station sums
-    constexpr int NST = 5;
-    const int nbg = (a->Nbase + 255) / 256;
-    int nsl = (db_sm_count() + nbg - 1) / nbg;
-    if (nsl > nt) nsl = nt;
-    ClusterPassArgs b = *a;
-    b.tslice = (nt + nsl - 1) / nsl;
-    const int forced = db_opt(DB_OPT_CP_ROWS);
-    if (forced > 0) b.tslice = forced;
-    if (b.tslice > nt) b.tslice = nt;
-    if (b.tslice > 32) b.tslice = 32;
-    const size_t smem = (size_t)NST * 8 * 256 * sizeof(double2) + sizeof(double) * ((8 * a->N + 1) & ~1) + NST * 8;
-    static bool configured = false;
-    if (!configured) {
-      DB_CHECK(cudaFuncSetAttribute(k_cluster_pass_lin<NST, false>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      configured = true;
-    }
-    dim3 glin(nbg, (nt + b.tslice - 1) / b.tslice);
-    k_cluster_pass_lin<NST, false><<<glin, 512, smem, st>>>(b);
-    return;
-  }
-  if (a->jte != nullptr && a->mode == 4) {
+  const bool fits = cluster_pass_lin_fits(a->N, a->Nbase);
+  if (a->jte == nullptr || (a->mode > 1 && a->mode != 4)) {
+    // ADD / SUB / cost-only pass: the linear mapping without the station sums, unless robust
+    // weights or a second input vector ask for the tile kernel
+    if (!a->wt && !a->in2 && fits) launch_cluster_pass_lin<false>(a, st);
+    else k_cluster_pass<<<grid, TILE_THREADS, 0, st>>>(*a);
+  } else if (a->mode == 4 || a->wt || !fits) {
     k_cluster_pass_split<<<grid, 2 * TILE_THREADS, 0, st>>>(*a);
-    return;
-  }
-  if (a->jte != nullptr && a->mode <= 1) {
-    static const bool unsplit = getenv("DIRAC_B200_CP_UNSPLIT") != nullptr;
-    // default: linear mapping with CTA-wide TMA stages; robust weights and DIRAC_B200_NO_TMA take the
-    // register-staged tile kernel
-    static const bool no_tma = getenv("DIRAC_B200_NO_TMA") != nullptr;
-    const bool lin_fits = cluster_pass_lin_fits(a->N, a->Nbase);
-    if (unsplit) {
-      k_cluster_pass<true><<<grid, TILE_THREADS, 0, st>>>(*a);
-    } else if (a->wt || no_tma || !lin_fits) {
-      k_cluster_pass_split<<<grid, 2 * TILE_THREADS, 0, st>>>(*a);
-    } else {
-      // linear mapping: 256 baselines per CTA, time sliced to about one CTA per SM (<= 32 rows)
-      constexpr int NST = 5;
-      const int nbg = (a->Nbase + 255) / 256;
-      int nsl = (db_sm_count() + nbg - 1) / nbg;
-      if (nsl > nt) nsl = nt;
-      ClusterPassArgs b = *a;
-      b.tslice = (nt + nsl - 1) / nsl;
-      // test hook: rows per CTA forced (drives the multi-row ring on small problems), as long as
-      // the slices still fit the per-CTA partial buffer
-      const int forced = db_opt(DB_OPT_CP_ROWS);
-      if (forced > 0 && (nt + forced - 1) / forced <= db_cp_max_slices(a->Nbase, nt)) b.tslice = forced;
-      if (b.tslice > nt) b.tslice = nt;
-      if (b.tslice > 32) b.tslice = 32;
-      const size_t smem = (size_t)NST * 8 * 256 * sizeof(double2) +
-                          sizeof(double) * ((8 * a->N + 1) & ~1) + NST * 8;
-      static bool configured = false;
-      if (!configured) {
-        DB_CHECK(cudaFuncSetAttribute(k_cluster_pass_lin<NST, true>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        configured = true;
-      }
-      dim3 glin(nbg, (nt + b.tslice - 1) / b.tslice);
-      k_cluster_pass_lin<NST, true><<<glin, 512, smem, st>>>(b);
-    }
   } else {
-    k_cluster_pass<false><<<grid, TILE_THREADS, 0, st>>>(*a);
+    launch_cluster_pass_lin<true>(a, st);
   }
 }
 void db_launch_coh_gram(const GramArgs *a, int ntile, int nk, cudaStream_t st) {

@@ -1,15 +1,16 @@
 // TMA-pipelined all-cluster passes (Blackwell/Hopper bulk-copy engine feeding a per-warp ring of
 // shared-memory stages):
-//   MODE 0  model over all clusters, residual / cost          (k_predict_full's job, lmfit.c:611-688)
-//   MODE 1  line model V0,V1,V2 -> E0,E1,E2 of the LBFGS line search      (k_line_setup's job)
+//   MODE 0  model over all clusters, residual / cost      (predict_threadfn_withgain_full,
+//           lmfit.c:611-688, plus cost_func / robust_cost_func, robust_lbfgs.c:674-726)
+//   MODE 1  line model V0,V1,V2 -> E0,E1,E2 of the LBFGS line search (kernels_line.cu)
 //
-// Why: the register-staged versions run 8 warps per SM (register bound) and expose the full DRAM
-// latency between dependent load->compute phases (ncu: 12.5 % warps active, DRAM 13-19 %, fp64 pipe
-// ~20 %; profiles/r01b_ncu_full_streaming_kernels.md).  Here one elected lane per warp issues 1-D
-// bulk copies (cp.async.bulk, 16 B x valid lanes = up to 512 B each) for the coherencies of the
-// NEXT cluster steps into the warp's private ring of NST shared-memory stages while the warp
-// multiplies the current one; no register is held by data in flight, several KB per warp are always
-// in flight, completion is tracked by one mbarrier per stage (complete_tx).  The warp is its own
+// Why a ring: a pass that loads the coherencies into registers holds them there until they are
+// used, so registers bound it to few resident warps, and each warp waits out the full DRAM latency
+// between its dependent load and compute phases.  Here one elected lane per warp issues 1-D bulk
+// copies (cp.async.bulk, 16 B x valid lanes = up to 512 B each) for the coherencies of the NEXT
+// cluster steps into the warp's private ring of NST shared-memory stages while the warp multiplies
+// the current one; no register is held by data in flight, several KB per warp are always in
+// flight, completion is tracked by one mbarrier per stage (complete_tx).  The warp is its own
 // producer and consumer, so no block-wide barrier appears in the main loop.
 //
 // Mapping: linear over the canonical baselines (no station reduction is needed by these passes):
@@ -19,7 +20,7 @@
 #include "internal.cuh"
 #include "tma.cuh"
 
-template <int MODE, int TB, int NST, int WARPS, bool PF>
+template <int MODE, int TB, int NST, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
 k_stream_all(StreamAllArgs a) {
   // One CTA = one item (32 consecutive baselines x TB timeslots); its WARPS warps split the clusters
@@ -81,10 +82,7 @@ k_stream_all(StreamAllArgs a) {
 #pragma unroll
     for (int c = 0; c < 4; c++) V0[i][c] = V1[i][c] = V2[i][c] = make_double2(0.0, 0.0);
 
-  // Jones of the first cluster of this warp; the next ones are fetched one step ahead so that their
-  // L1/L2 latency hides behind the 2x2 products of the current step
   double2 Jp[4], Jq[4], Dp[4], Dq[4];
-  double2 nJp[4], nJq[4], nDp[4], nDq[4];
   auto fetch_jones = [&](int j, double2 *jp, double2 *jq, double2 *dp, double2 *dq) {
     const int k = w + j * WARPS;
     const ClusterDesc cd = a.clus[k];
@@ -97,21 +95,11 @@ k_stream_all(StreamAllArgs a) {
       load_jones(a.pk + off, q, dq);
     }
   };
-  if (PF && nk > 0) fetch_jones(0, nJp, nJq, nDp, nDq);
 
   for (int j = 0; j < nk; j++) {
     const int s = j % NST;
     if (lane == 0 && j + NST - 1 < nk) issue(j + NST - 1, (j + NST - 1) % NST);
-    if (PF) {
-#pragma unroll
-      for (int c = 0; c < 4; c++) {
-        Jp[c] = nJp[c]; Jq[c] = nJq[c];
-        if (MODE == 1) { Dp[c] = nDp[c]; Dq[c] = nDq[c]; }
-      }
-      if (j + 1 < nk) fetch_jones(j + 1, nJp, nJq, nDp, nDq);
-    } else {
-      fetch_jones(j, Jp, Jq, Dp, Dq);
-    }
+    fetch_jones(j, Jp, Jq, Dp, Dq);
     const int k = w + j * WARPS;
     const ClusterDesc cd = a.clus[k];
     mbar_wait(&my_bar[s], (unsigned)((j / NST) & 1));
@@ -241,14 +229,9 @@ k_stream_all(StreamAllArgs a) {
 }
 
 // ---- launchers ---------------------------------------------------------------------------------------
-#define SA_WARPS 3
-#define SA_NST 2
-#define SA_TB0 2  // predict
-#define SA_TB1 2  // line setup
-
 static int g_line_shape[3] = {-1, -1, -1};  // shape of the last line-model launch (tests)
 
-template <int MODE, int TB, int NST, int WARPS, bool PF>
+template <int MODE, int TB, int NST, int WARPS>
 static void launch_cfg(const StreamAllArgs *a, cudaStream_t st) {
   if (MODE == 1) {
     g_line_shape[0] = TB;
@@ -263,75 +246,11 @@ static void launch_cfg(const StreamAllArgs *a, cudaStream_t st) {
   const size_t smem = (ring > comb ? ring : comb) + WARPS * NST * 8;
   static bool configured = false;
   if (!configured) {
-    DB_CHECK(cudaFuncSetAttribute(k_stream_all<MODE, TB, NST, WARPS, PF>,
+    DB_CHECK(cudaFuncSetAttribute(k_stream_all<MODE, TB, NST, WARPS>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  k_stream_all<MODE, TB, NST, WARPS, PF><<<grid, WARPS * 32, smem, st>>>(*a);
-}
-
-// tuning hook: DIRAC_B200_SA_CFG selects one of the compiled shapes (TB rows, NST stages, WARPS)
-static int sa_cfg() {
-  static int v = -1;
-  if (v < 0) {
-    const char *e = getenv("DIRAC_B200_SA_CFG");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-template <int MODE, int TB>
-static void launch_stream_all(const StreamAllArgs *a, cudaStream_t st) {
-  if (MODE == 0) {
-    switch (sa_cfg()) {
-      case 1: launch_cfg<MODE, 2, 2, 4, false>(a, st); return;
-      case 2: launch_cfg<MODE, 2, 2, 2, false>(a, st); return;
-      case 3: launch_cfg<MODE, 2, 3, 3, false>(a, st); return;
-      case 4: launch_cfg<MODE, 4, 2, 3, false>(a, st); return;
-      case 5: launch_cfg<MODE, 4, 2, 4, false>(a, st); return;
-      case 6: launch_cfg<MODE, 1, 2, 3, false>(a, st); return;
-      case 7: launch_cfg<MODE, 3, 2, 3, false>(a, st); return;
-      case 8: launch_cfg<MODE, 2, 2, 3, true>(a, st); return;
-      case 9: launch_cfg<MODE, 2, 2, 4, true>(a, st); return;
-      case 10: launch_cfg<MODE, 2, 2, 2, true>(a, st); return;
-      case 11: launch_cfg<MODE, 4, 2, 3, true>(a, st); return;
-      default: break;
-    }
-  }
-  if (MODE == 1) {
-    static int v1 = -1;
-    if (v1 < 0) {
-      const char *e = getenv("DIRAC_B200_SA_CFG1");
-      v1 = e ? atoi(e) : 0;
-    }
-    if (v1 == 0) {
-      // one row per item keeps the three accumulated polynomials of the line model at 24 registers
-      // pairs (222 -> ~170 registers: 7.5 % -> 12 % resident warps, ncu r02).  Splitting the clusters
-      // of an item over warps only pays while the grid is short of warps (62 stations: 7200 items);
-      // a large array has plenty (512 stations: 490 k items) and skips the cross-warp combine.
-      const long long items = (long long)((a->Nbase + 31) / 32) * a->tilesz;
-      if (items >= 64ll * db_sm_count()) launch_cfg<MODE, 1, 4, 1, false>(a, st);
-      else launch_cfg<MODE, 1, 2, 3, false>(a, st);
-      return;
-    }
-    switch (v1) {
-      case 1: launch_cfg<MODE, 2, 2, 3, false>(a, st); return;
-      case 2: launch_cfg<MODE, 1, 3, 3, false>(a, st); return;
-      case 3: launch_cfg<MODE, 1, 2, 4, false>(a, st); return;
-      case 4: launch_cfg<MODE, 1, 3, 4, false>(a, st); return;
-      case 5: launch_cfg<MODE, 2, 2, 4, false>(a, st); return;
-      case 6: launch_cfg<MODE, 1, 4, 2, false>(a, st); return;
-      case 7: launch_cfg<MODE, 1, 2, 6, false>(a, st); return;
-      case 8: launch_cfg<MODE, 1, 2, 8, false>(a, st); return;
-      case 9: launch_cfg<MODE, 1, 4, 1, false>(a, st); return;
-      case 10: launch_cfg<MODE, 1, 6, 1, false>(a, st); return;
-      case 11: launch_cfg<MODE, 1, 6, 2, false>(a, st); return;
-      case 12: launch_cfg<MODE, 1, 8, 2, false>(a, st); return;
-      case 13: launch_cfg<MODE, 2, 4, 2, false>(a, st); return;
-      case 14: launch_cfg<MODE, 1, 3, 2, false>(a, st); return;
-      default: break;
-    }
-  }
-  launch_cfg<MODE, TB, SA_NST, SA_WARPS, false>(a, st);
+  k_stream_all<MODE, TB, NST, WARPS><<<grid, WARPS * 32, smem, st>>>(*a);
 }
 
 extern "C" {
@@ -341,10 +260,16 @@ int db_stream_all_nblocks(int Nbase, int tilesz) {
   return (int)((long long)nbg * tilesz);
 }
 void db_launch_predict_tma(const StreamAllArgs *a, cudaStream_t st) {
-  launch_stream_all<0, SA_TB0>(a, st);
+  launch_cfg<0, 2, 2, 3>(a, st);
 }
 void db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st) {
-  launch_stream_all<1, SA_TB1>(a, st);
+  // one row per item keeps the three accumulated polynomials of the line model at 24 registers
+  // pairs (222 -> ~170 registers: 7.5 % -> 12 % resident warps, ncu r02).  Splitting the clusters
+  // of an item over warps only pays while the grid is short of warps (62 stations: 7200 items);
+  // a large array has plenty (512 stations: 490 k items) and skips the cross-warp combine.
+  const long long items = (long long)((a->Nbase + 31) / 32) * a->tilesz;
+  if (items >= 64ll * db_sm_count()) launch_cfg<1, 1, 4, 1>(a, st);
+  else launch_cfg<1, 1, 2, 3>(a, st);
 }
 void db_line_setup_shape_reset() { g_line_shape[0] = g_line_shape[1] = g_line_shape[2] = -1; }
 void db_line_setup_shape(int *shape) {

@@ -8,10 +8,10 @@
 // What differs is the cost of a cost evaluation.  Every evaluation of the reference's line search
 // is at x_k + alpha p_k (the reference moves a scratch vector xp along p_k by axpy; we track the
 // same alpha with the same sequence of additions).  One pass over the coherencies per LBFGS
-// iteration (k_line_setup) leaves the line model e(alpha) = E0 - alpha E1 - alpha^2 E2 in HBM/L2;
+// iteration (k_stream_all<1>) leaves the line model e(alpha) = E0 - alpha E1 - alpha^2 E2 in HBM/L2;
 // each of the 10-30 cost evaluations of the iteration is then a 192 B/row reduction (k_line_eval)
 // instead of a full predict over all clusters, and the residual at the accepted step feeds the
-// gradient pass (k_grad_full) directly.  Per iteration: 2 passes over the coherencies instead of
+// gradient pass (k_grad_tma_split) directly.  Per iteration: 2 passes over the coherencies instead of
 // ~30 (cost_func / robust_cost_func, robust_lbfgs.c:674-726; func_grad(_robust), :569-669,322-416).
 //
 // The iterate, the gradient, the search direction and the (s, y) history live on the device; the
@@ -33,7 +33,6 @@ void db_launch_lbfgs_step(const double *xk, const double *pk, const double *gk, 
                           double *sk, double *yk, int m, double alpha, cudaStream_t st);
 void db_launch_lbfgs_update(const double *gk, const double *sk, double *yk, const double *xk1,
                             double *xk, int m, double *rho_slot, double *out, cudaStream_t st);
-void db_launch_line_setup(const LineSetupArgs *a, int ntile, cudaStream_t st);
 void db_launch_line_eval(const double2 *E0, const double2 *E1, const double2 *E2, long long n4,
                          double alpha, int mode, double inv_nu, double *partials, double *out,
                          unsigned int *counter, cudaStream_t st);
@@ -67,17 +66,13 @@ static void line_setup(LbfgsCtx *c, const double *xk, const double *pk) {
   dirac_b200_problem *pr = c->pr;
   DevProblem &d = pr->d;
   line_alloc(pr);
-  LineSetupArgs a;
-  a.coh = d.coh; a.x = d.x; a.flag = d.flag; a.xk = xk; a.pk = pk; a.clus = d.clus;
-  a.chunk_poff = d.chunk_poff; a.tiles = d.tiles; a.E0 = pr->E0; a.E1 = pr->E1; a.E2 = pr->E2;
-  a.R = d.R; a.N = d.N; a.Nbase = d.Nbase; a.tilesz = d.tilesz; a.M = d.M;
-  a.partial = (pr->world > 1) ? 1 : 0;
   StreamAllArgs s;
   memset(&s, 0, sizeof(s));
-  s.coh = a.coh; s.x = a.x; s.flag = a.flag; s.pp = a.xk; s.pk = a.pk; s.clus = a.clus;
-  s.chunk_poff = a.chunk_poff; s.blpq = d.blpq; s.E0 = a.E0; s.E1 = a.E1; s.E2 = a.E2;
-  s.R = a.R; s.N = a.N; s.Nbase = a.Nbase; s.tilesz = a.tilesz; s.M = a.M; s.partial = a.partial;
-  if (db_use_tma() && db_overlap_available(pr) && d.tilesz >= 8) {
+  s.coh = d.coh; s.x = d.x; s.flag = d.flag; s.pp = xk; s.pk = pk; s.clus = d.clus;
+  s.chunk_poff = d.chunk_poff; s.blpq = d.blpq; s.E0 = pr->E0; s.E1 = pr->E1; s.E2 = pr->E2;
+  s.R = d.R; s.N = d.N; s.Nbase = d.Nbase; s.tilesz = d.tilesz; s.M = d.M;
+  s.partial = (pr->world > 1) ? 1 : 0;  // 1: the raw sums V0,V1,V2 of the local clusters
+  if (db_overlap_available(pr) && d.tilesz >= 8) {
     // Sharded: the kernel runs in time chunks; each chunk's 12 slices (3 vectors x 4 polarisation
     // planes) are summed over the ranks on the communication stream while the next chunk is computed
     static cudaEvent_t ev_chunk[8], ev_done;
@@ -120,8 +115,7 @@ static void line_setup(LbfgsCtx *c, const double *xk, const double *pk) {
     db_count_launch(1);
   } else {
     db_prof_begin(7, (double)d.R * (64.0 * d.M + 65.0 + 192.0), d.stream);
-    if (db_use_tma()) db_launch_line_setup_tma(&s, d.stream);
-    else db_launch_line_setup(&a, d.ntile, d.stream);
+    db_launch_line_setup_tma(&s, d.stream);
     db_prof_end(d.stream);
     db_count_launch(1);
     if (pr->world > 1) {
@@ -382,8 +376,7 @@ void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, in
 //   poly    the 5 coefficients of the Gaussian cost along the line (k_line_poly)
 //   costs   [2 * nalpha]: k_line_eval at alphas[i], Gaussian (2i) and Student's-t with nu (2i + 1)
 //   res     8R doubles: k_line_residual at alpha_res, API layout
-//   shape   (TB, NST, WARPS) of the k_stream_all<1> launch that ran, or (0, 0, 0) for the
-//           register-staged k_line_setup (DIRAC_B200_NO_TMA)
+//   shape   (TB, NST, WARPS) of the k_stream_all<1> launch that ran
 extern "C" void dirac_b200_line_model(dirac_b200_problem *pr, const double *xk, const double *pk,
                                       int nalpha, const double *alphas, double nu,
                                       double alpha_res, double *E, double *poly, double *costs,
@@ -397,8 +390,7 @@ extern "C" void dirac_b200_line_model(dirac_b200_problem *pr, const double *xk, 
   DB_CHECK(cudaMemcpyAsync(dp, pk, sizeof(double) * d.npar, cudaMemcpyHostToDevice, d.stream));
   db_line_setup_shape_reset();
   line_setup(&c, dx, dp);
-  if (db_use_tma()) db_line_setup_shape(shape);
-  else shape[0] = shape[1] = shape[2] = 0;
+  db_line_setup_shape(shape);
   for (int j = 0; j < 5; j++) poly[j] = c.poly[j];
   for (int i = 0; i < nalpha; i++)
     for (int mode = 1; mode <= 2; mode++) {
@@ -413,25 +405,4 @@ extern "C" void dirac_b200_line_model(dirac_b200_problem *pr, const double *xk, 
   db_download_vis(pr, pr->res, res);
   DB_CHECK(cudaGetLastError());
   db_free(dx);
-}
-
-// micro-benchmark of the line-model setup on the resident problem (direction = current Jones):
-// average device time (us) of `reps` back-to-back launches
-extern "C" double dirac_b200_bench_line_setup(dirac_b200_problem *pr, int reps) {
-  DevProblem &d = pr->d;
-  LbfgsCtx c;
-  c.pr = pr; c.robust = 1; c.nu = 2.0; c.m = (int)d.npar; c.ncost = c.ngrad = 0;
-  cudaEvent_t e0, e1;
-  DB_CHECK(cudaEventCreate(&e0));
-  DB_CHECK(cudaEventCreate(&e1));
-  for (int i = 0; i < 2; i++) line_setup(&c, d.pp, d.pp);
-  DB_CHECK(cudaEventRecord(e0, d.stream));
-  for (int i = 0; i < reps; i++) line_setup(&c, d.pp, d.pp);
-  DB_CHECK(cudaEventRecord(e1, d.stream));
-  DB_CHECK(cudaEventSynchronize(e1));
-  float ms = 0.f;
-  DB_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  return 1e3 * ms / reps;
 }

@@ -176,9 +176,7 @@ void db_lm_free(dirac_b200_problem *pr) {
 
 // timeslots per CTA slice of a per-cluster pass: enough slices to fill the GPU, long enough to
 // amortise the per-slice station reduction
-static int g_tslice_override = 0;  // tuning hook (dirac_b200_bench_cluster_pass)
 static int pick_tslice(const DevProblem &d, int nt) {
-  if (g_tslice_override > 0) return g_tslice_override < nt ? g_tslice_override : nt;
   int target_ctas = db_sm_count();  // one wave: these kernels run 1 CTA per SM (register bound)
   int slices = (target_ctas + d.ntile - 1) / d.ntile;
   if (slices < 1) slices = 1;
@@ -216,7 +214,7 @@ void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, cons
   a.mode = mode; a.write_out = write_out; a.wt = wt; a.beta = beta; a.in2 = in2;
   a.pblk_old = pblk_old; a.form_hidden = form_hidden;
   // passes without the gradient accumulator fit two CTAs per SM: twice as many, half as long
-  if (!(jte_dev && (mode <= 1 || mode == 4)) && g_tslice_override <= 0 && a.tslice > 1)
+  if (!(jte_dev && (mode <= 1 || mode == 4)) && a.tslice > 1)
     a.tslice = (a.tslice + 1) / 2;
   if (jte_dev && (mode <= 1 || mode == 4) && !jte_zeroed)
     DB_CHECK(cudaMemsetAsync(jte_dev, 0, sizeof(double) * 8 * d.N, d.stream));
@@ -1420,14 +1418,12 @@ extern "C" double dirac_b200_bench_grad(dirac_b200_problem *pr, int reps) {
 
 // micro-benchmark of one k_cluster_pass configuration on the resident problem: average device time
 // (us, CUDA events on the launching stream) of `reps` back-to-back launches over the full interval.
-// with_grad: also accumulate J^T e; write_out: write the residual; tslice <= 0: default slicing.
+// with_grad: also accumulate J^T e; write_out: write the residual.
 extern "C" double dirac_b200_bench_cluster_pass(dirac_b200_problem *pr, int clus, int mode,
-                                                int with_grad, int write_out, int tslice,
-                                                int reps) {
+                                                int with_grad, int write_out, int reps) {
   DevProblem &d = pr->d;
   db_lm_init(pr);
   LMWork &w = pr->lm;
-  g_tslice_override = tslice;
   double *pblk = d.pp + d.h_chunk_poff[d.h_clus[clus].chunk0];
   cudaEvent_t e0, e1;
   DB_CHECK(cudaEventCreate(&e0));
@@ -1445,6 +1441,5 @@ extern "C" double dirac_b200_bench_cluster_pass(dirac_b200_problem *pr, int clus
   DB_CHECK(cudaEventElapsedTime(&ms, e0, e1));
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
-  g_tslice_override = 0;
   return 1e3 * ms / reps;
 }

@@ -363,10 +363,9 @@ static dirac_b200_problem *create_impl(int N, int Nbase, int tilesz, const basel
   }
 
   // --- scratch ---
-  int nb1 = db_predict_nblocks(d.ntile, tilesz);
-  int nb2 = db_cluster_pass_nblocks(d.ntile, tilesz, 1);
+  const int nb2 = db_cluster_pass_nblocks(d.ntile, tilesz, 1);
   const int nb3 = db_stream_all_nblocks(Nbase, tilesz);
-  pr->npartials = (nb1 > nb2 ? (nb1 > nb3 ? nb1 : nb3) : (nb2 > nb3 ? nb2 : nb3)) + 1024;  // also covers the fixed-grid reductions
+  pr->npartials = (nb2 > nb3 ? nb2 : nb3) + 1024;  // also covers the fixed-grid reductions
   pr->partials = dev_alloc<double>(pr->npartials);
   // scalars [0,64) followed by the LM mailbox (step, J^T e at two points, solver status): everything
   // the host needs after a trial comes back in ONE device-to-host copy
@@ -442,35 +441,13 @@ extern "C" void dirac_b200_get_coherencies(dirac_b200_problem *pr, double *coh) 
 // ------------------------------------------------------------------------------------------------
 // model/residual/cost over all clusters at the Jones currently in d.pp; returns after queuing;
 // the cost lands in d.scal[slot] (device)
-// TMA-pipelined kernels unless DIRAC_B200_NO_TMA is set (A/B comparison, fallback for debugging)
-int db_use_tma() {
-  static int v = -1;
-  if (v < 0) v = getenv("DIRAC_B200_NO_TMA") ? 0 : 1;
-  return v;
-}
-
-static void predict_launch(dirac_b200_problem *pr, const PredictArgs &a) {
-  DevProblem &d = pr->d;
-  if (db_use_tma()) {
-    StreamAllArgs s;
-    memset(&s, 0, sizeof(s));
-    s.coh = a.coh; s.x = a.x; s.flag = a.flag; s.pp = a.pp; s.clus = a.clus;
-    s.chunk_poff = a.chunk_poff; s.blpq = d.blpq; s.out = a.out; s.partials = a.partials;
-    s.cost = a.cost; s.counter = a.counter; s.R = a.R; s.N = a.N; s.Nbase = a.Nbase;
-    s.tilesz = a.tilesz; s.M = a.M; s.out_mode = a.out_mode; s.cost_mode = a.cost_mode;
-    s.inv_nu = a.inv_nu;
-    db_launch_predict_tma(&s, d.stream);
-  } else {
-    db_launch_predict_full(&a, d.ntile, d.stream);
-  }
-}
-
 void db_predict_dev(dirac_b200_problem *pr, const double *pp_dev, double2 *out, int out_mode,
                     int cost_mode, double nu, int slot) {
   DevProblem &d = pr->d;
-  PredictArgs a;
+  StreamAllArgs a;
+  memset(&a, 0, sizeof(a));
   a.coh = d.coh; a.x = d.x; a.flag = d.flag; a.pp = pp_dev; a.clus = d.clus;
-  a.chunk_poff = d.chunk_poff; a.tiles = d.tiles; a.out = out; a.partials = pr->partials;
+  a.chunk_poff = d.chunk_poff; a.blpq = d.blpq; a.out = out; a.partials = pr->partials;
   a.cost = d.scal + slot; a.counter = d.counters; a.R = d.R; a.N = d.N; a.Nbase = d.Nbase;
   a.tilesz = d.tilesz; a.M = d.M; a.out_mode = out_mode; a.cost_mode = cost_mode;
   a.inv_nu = (nu > 0.0) ? 1.0 / nu : 0.0;
@@ -480,7 +457,7 @@ void db_predict_dev(dirac_b200_problem *pr, const double *pp_dev, double2 *out, 
     if (!pr->pm) pr->pm = dev_alloc<double2>((size_t)4 * d.R);
     a.out = pr->pm; a.out_mode = 2; a.cost_mode = 0;
     db_prof_begin(0, (double)d.R * (64.0 * d.M + 65.0 + 64.0), d.stream);
-    predict_launch(pr, a);
+    db_launch_predict_tma(&a, d.stream);
     db_prof_end(d.stream);
     db_allreduce(pr, pr->pm, 8 * d.R);
     db_launch_residual_cost(d.x, pr->pm, out, 4 * d.R, out ? out_mode : 0, cost_mode, a.inv_nu,
@@ -489,7 +466,7 @@ void db_predict_dev(dirac_b200_problem *pr, const double *pp_dev, double2 *out, 
     return;
   }
   db_prof_begin(0, (double)d.R * (64.0 * d.M + 65.0 + (out_mode ? 64.0 : 0.0)), d.stream);
-  predict_launch(pr, a);
+  db_launch_predict_tma(&a, d.stream);
   db_prof_end(d.stream);
   db_count_launch(1);
 }
@@ -515,8 +492,7 @@ void db_grad_dev(dirac_b200_problem *pr, const double *pp_dev, double *g_dev, in
   // robust g = +2 (f-d) df/(nu+(f-d)^2) (robust_lbfgs.c:286-299); here e = d-f
   a.scale = robust ? -2.0 : 2.0;
   db_prof_begin(1, (double)d.R * (64.0 * d.M + 65.0) + 64.0 * d.N * d.Mt, d.stream);
-  if (db_use_tma()) db_launch_grad_tma(&a, d.ntile, d.stream);
-  else db_launch_grad_full(&a, d.ntile, d.stream);
+  db_launch_grad_tma(&a, d.ntile, d.stream);
   db_prof_end(d.stream);
   db_count_launch(1);
   // sharded: every rank filled the blocks of its own clusters; the sum is the full gradient

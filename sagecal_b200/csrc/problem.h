@@ -100,7 +100,6 @@ void db_predict_dev(dirac_b200_problem *pr, const double *pp_dev, double2 *out, 
 double db_read_scalar(dirac_b200_problem *pr, int slot);
 void db_grad_dev(dirac_b200_problem *pr, const double *pp_dev, double *g_dev, int robust,
                  double nu);
-int db_use_tma();
 void db_lm_init(dirac_b200_problem *pr);
 void db_prefactor_sweep(dirac_b200_problem *pr, double tau);
 void db_allreduce(dirac_b200_problem *pr, void *dev, long long count);

@@ -186,8 +186,7 @@ class DeviceProblem:
     def line_model(self, xk, pk, alphas, nu, alpha_res):
         """the LBFGS line model along pk from xk as one iteration sets it up (dirac_b200_line_model).
         returns dict(E0, E1, E2 [API layout], poly [5], cost_gauss, cost_robust [per alpha],
-        res [line residual at alpha_res], shape (TB, NST, WARPS) of the k_stream_all<1> launch or
-        (0, 0, 0) for the register-staged k_line_setup)"""
+        res [line residual at alpha_res], shape (TB, NST, WARPS) of the k_stream_all<1> launch)"""
         L = self.api.lib
         L.dirac_b200_line_model.restype = None
         L.dirac_b200_line_model.argtypes = [C.c_void_p, c_double_p, c_double_p, C.c_int, c_double_p,

@@ -1,5 +1,5 @@
 """Run one small sagefit solve and dump the solved Jones + residual norms (stdout, JSON).  Executed in
-a subprocess by test_gpu_solvers.py with different DIRAC_B200_* switches: the library reads them once
+a subprocess by test_gpu_solvers.py with and without DIRAC_B200_CUSOLVER: the library reads it once
 per process."""
 import json
 import os

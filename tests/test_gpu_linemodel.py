@@ -1,4 +1,4 @@
-"""The LBFGS line model (E0, E1, E2 of k_stream_all<1> / k_line_setup), its quartic (k_line_poly),
+"""The LBFGS line model (E0, E1, E2 of k_stream_all<1>), its quartic (k_line_poly),
 the direct line costs (k_line_eval) and the line residual (k_line_residual) against a plain numpy
 restatement, in both launch shapes of k_stream_all<1>.
 
@@ -6,19 +6,19 @@ k_stream_all<1> runs one warp per item with a 4-stage ring once the grid has at 
 (32 baselines x 1 timeslot) per SM, and three warps per item with a cross-warp combine below that.
 The solver's line search differentiates its costs numerically, so a wrong E1 or E2 could still let
 a whole LBFGS run find some step: these tests read the line model directly."""
-import json
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-from linemodel_check import ALPHA_RES, ALPHAS, NU, make_case, run_case
-from util import line_model_ref, lsum, relerr
+from sagecal_b200 import lib as blib
+from util import line_model_ref, lsum, relerr, small_problem
 
 pytestmark = pytest.mark.gpu
+
+ALPHAS = np.array([0.0, 1e-6, 0.37, 1.0, -0.5, 3.0])
+NU = 3.5
+ALPHA_RES = 0.63
 
 SMALL_SHAPE = (1, 2, 3)   # (TB, NST, WARPS) below 64 items per SM
 LARGE_SHAPE = (1, 4, 1)   # at or above
@@ -53,6 +53,22 @@ def _case(name):
     if case["tilesz"] is None:
         case["tilesz"] = _large_tilesz(case["N"])
     return case, shape
+
+
+def make_case(case):
+    """(bound problem, xk, pk) of a case dict: N, M, tilesz, seed, optional nchunk / kmean"""
+    kw = {k: v for k, v in case.items() if k in ("nchunk", "kmean")}
+    b = small_problem(N=case["N"], M=case["M"], tilesz=case["tilesz"], seed=case["seed"], **kw)
+    rng = np.random.default_rng(case["seed"] + 1000)
+    xk = b.pr.pp0 + 0.1 * rng.normal(0, 1, b.pr.pp0.shape)
+    pk = 0.05 * rng.normal(0, 1, b.pr.pp0.shape)
+    return b, xk, pk
+
+
+def run_case(api, b, xk, pk):
+    pr = b.pr
+    with blib.DeviceProblem(api, pr.N, pr.Nbase, pr.tilesz, b.barr, b.sky, pr.coh, pr.x) as dp:
+        return dp.line_model(xk, pk, ALPHAS, NU, ALPHA_RES)
 
 
 def check_line_model(b, xk, pk, got):
@@ -102,18 +118,3 @@ def test_line_model(api, name):
     assert got["shape"] == shape, (name, items, got["shape"])
     check_line_model(b, xk, pk, got)
 
-
-def test_line_model_register_staged(api, tmp_path):
-    """k_line_setup, the register-staged line model (DIRAC_B200_NO_TMA=1), in a process of its own"""
-    case, _ = _case("small-hybrid")
-    script = os.path.join(os.path.dirname(os.path.abspath(__file__)), "linemodel_check.py")
-    env = dict(os.environ)
-    env["DIRAC_B200_NO_TMA"] = "1"
-    out_path = str(tmp_path / "line.npz")
-    out = subprocess.run([sys.executable, script, json.dumps(case), out_path], env=env,
-                         capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    z = np.load(out_path)
-    got = {k: z[k] for k in z.files}
-    assert tuple(got.pop("shape")) == (0, 0, 0)
-    check_line_model(*make_case(case), got)

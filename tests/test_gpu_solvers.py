@@ -89,11 +89,10 @@ def test_index_helpers_bit_exact(api, ref):
     assert np.array_equal(res[0][0], res[1][0]) and np.array_equal(res[0][1], res[1][1])
 
 
-@pytest.mark.parametrize("switch", ["DIRAC_B200_CUSOLVER", "DIRAC_B200_NO_TMA", "DIRAC_B200_CP_UNSPLIT"])
+@pytest.mark.parametrize("switch", ["DIRAC_B200_CUSOLVER"])
 def test_alternate_paths_agree(api, switch):
-    """The library fallbacks (cuSOLVER instead of the cluster Cholesky, register-staged instead of
-    TMA-fed kernels, unsplit gradient pass) solve the same problem to the same Jones: they differ in
-    summation order only."""
+    """The library fallback (cuSOLVER instead of the cluster Cholesky) solves the same problem to the
+    same Jones: the two differ in summation order only."""
     import json
     import os
     import subprocess
@@ -102,8 +101,7 @@ def test_alternate_paths_agree(api, switch):
 
     def run(env_extra):
         env = dict(os.environ)
-        for k in ("DIRAC_B200_CUSOLVER", "DIRAC_B200_NO_TMA", "DIRAC_B200_CP_UNSPLIT"):
-            env.pop(k, None)
+        env.pop("DIRAC_B200_CUSOLVER", None)
         env.update(env_extra)
         out = subprocess.run([sys.executable, script], env=env, capture_output=True, text=True,
                              timeout=600)
