@@ -699,8 +699,25 @@ typedef struct {
   const double *x;
   int robust;
   double nu;
+  long long ncost;  /* cost evaluations so far */
+  double margin;    /* smallest decision margin so far, in units of its rounding noise */
 } lb_ctx;
-static double lb_cost(lb_ctx *c, const double *p) { return orc_cost(c->P, p, c->x, c->robust, c->nu); }
+static double lb_cost(lb_ctx *c, const double *p) {
+  c->ncost++;
+  return orc_cost(c->P, p, c->x, c->robust, c->nu);
+}
+/* One comparison lhs <op> rhs of the line search: its margin |lhs - rhs| over `noise`, the change of
+ * lhs - rhs that rounding of the costs behind it can cause (costs known to eps |cost|, a central
+ * difference of two costs to eps (|p01| + |p02|) / (2 step)).  The smallest margin of a run says how
+ * far every decision was from flipping under a cost computed another way (the product's quartic). */
+static void lb_decide(lb_ctx *c, double lhs, double rhs, double noise) {
+  if (noise > 0.0 && fabs(lhs - rhs) / noise < c->margin) c->margin = fabs(lhs - rhs) / noise;
+}
+#define LB_EPS DBL_EPSILON
+static double cost_noise(double a, double b) { return LB_EPS * (fabs(a) + fabs(b)); }
+static double diff_noise(double p01, double p02, double step) {
+  return LB_EPS * (fabs(p01) + fabs(p02)) / (2.0 * step);
+}
 static double vdot(const double *a, const double *b, int m) {
   double s = 0.0;
   for (int i = 0; i < m; i++) s += a[i] * b[i];
@@ -710,8 +727,8 @@ static void vaxpy(double *y, const double *x, double a, int m) {
   for (int i = 0; i < m; i++) y[i] += a * x[i];
 }
 
-static void mult_hessian(int m, double *pk, const double *gk, const double *s, const double *y,
-                         const double *rho, int M, int ii) {
+void orc_mult_hessian(int m, double *pk, const double *gk, const double *s, const double *y,
+                      const double *rho, int M, int ii) {
   double *alphai = (double *)xcalloc(M, sizeof(double));
   int *idx = (int *)xcalloc(M, sizeof(int));
   if (M > 0) {
@@ -751,6 +768,7 @@ static double cubic_interp(lb_ctx *c, const double *xk, const double *pk, double
   vaxpy(xp, pk, -2.0 * step, m);
   p02 = lb_cost(c, xp);
   f0d = (p01 - p02) / (2.0 * step);
+  const double d0 = diff_noise(p01, p02, step);
   vaxpy(xp, pk, -a + step + b, m);
   f1 = lb_cost(c, xp);
   vaxpy(xp, pk, step, m);
@@ -758,29 +776,42 @@ static double cubic_interp(lb_ctx *c, const double *xk, const double *pk, double
   vaxpy(xp, pk, -2.0 * step, m);
   p02 = lb_cost(c, xp);
   f1d = (p01 - p02) / (2.0 * step);
+  const double d1 = diff_noise(p01, p02, step);
   aa = 3.0 * (f0 - f1) / (b - a) + (f1d - f0d);
   p01 = aa * aa - f0d * f1d;
+  const double na = 3.0 * cost_noise(f0, f1) / fabs(b - a) + d0 + d1;
+  lb_decide(c, p01, 0.0, 2.0 * fabs(aa) * na + fabs(f1d) * d0 + fabs(f0d) * d1);
   if (p01 > 0.0) {
+    const double nd = 2.0 * fabs(aa) * na + fabs(f1d) * d0 + fabs(f0d) * d1;
     cc = sqrt(p01);
-    z0 = b - (f1d + cc - aa) * (b - a) / (f1d - f0d + 2.0 * cc);
+    const double num = f1d + cc - aa, den = f1d - f0d + 2.0 * cc, ncc = nd / (2.0 * cc);
+    z0 = b - num * (b - a) / den;
+    const double nz = fabs(b - a) * ((d1 + ncc + na) / fabs(den) + fabs(num) * (d0 + d1 + 2.0 * ncc) /
+                                     (den * den));
     aa = (a > b) ? a : b;
     cc = (a < b) ? a : b;
+    lb_decide(c, z0, aa, nz);
+    if (!(z0 > aa)) lb_decide(c, z0, cc, nz);
     if (z0 > aa || z0 < cc) {
       fz0 = f0 + f1;
     } else {
       vaxpy(xp, pk, -b + step + a + z0 * (b - a), m);
       fz0 = lb_cost(c, xp);
     }
+    lb_decide(c, f0, f1, cost_noise(f0, f1));
+    if (f0 < f1) lb_decide(c, f0, fz0, cost_noise(f0, fz0));
     if (f0 < f1 && f0 < fz0) return a;
+    lb_decide(c, f1, fz0, cost_noise(f1, fz0));
     if (f1 < fz0) return b;
     return z0;
   }
+  lb_decide(c, f0, f1, cost_noise(f0, f1));
   return (f0 < f1) ? a : b;
 }
 
 static double ls_zoom(lb_ctx *c, const double *xk, const double *pk, double a, double b, double *xp,
-                      double phi_0, double gphi_0, double sigma, double rho, double t2, double t3,
-                      int m, double step) {
+                      double phi_0, double gphi_0, double n0, double sigma, double rho, double t2,
+                      double t3, int m, double step) {
   double alphaj = 0.0, phi_j, phi_aj, gphi_j, p01, p02, aj = a, bj = b, alphak = 1.0;
   int ci = 0, found = 0;
   while (ci < 10) {
@@ -792,6 +823,9 @@ static double ls_zoom(lb_ctx *c, const double *xk, const double *pk, double a, d
     phi_j = lb_cost(c, xp);
     vaxpy(xp, pk, -alphaj + aj, m);
     phi_aj = lb_cost(c, xp);
+    lb_decide(c, phi_j, phi_0 + rho * alphaj * gphi_0,
+              cost_noise(phi_j, phi_0) + rho * fabs(alphaj) * n0);
+    if (!(phi_j > phi_0 + rho * alphaj * gphi_0)) lb_decide(c, phi_j, phi_aj, cost_noise(phi_j, phi_aj));
     if ((phi_j > phi_0 + rho * alphaj * gphi_0) || phi_j >= phi_aj) {
       bj = alphaj;
     } else {
@@ -800,16 +834,20 @@ static double ls_zoom(lb_ctx *c, const double *xk, const double *pk, double a, d
       vaxpy(xp, pk, -2.0 * step, m);
       p02 = lb_cost(c, xp);
       gphi_j = (p01 - p02) / (2.0 * step);
+      const double nj = diff_noise(p01, p02, step);
+      lb_decide(c, (aj - alphaj) * gphi_j, step, fabs(aj - alphaj) * nj);
       if ((aj - alphaj) * gphi_j <= step) {
         alphak = alphaj;
         found = 1;
         break;
       }
+      lb_decide(c, fabs(gphi_j), -sigma * gphi_0, nj + sigma * n0);
       if (fabs(gphi_j) <= -sigma * gphi_0) {
         alphak = alphaj;
         found = 1;
         break;
       }
+      lb_decide(c, gphi_j * (bj - aj), 0.0, fabs(bj - aj) * nj);
       if (gphi_j * (bj - aj) >= 0) bj = aj;
       aj = alphaj;
     }
@@ -832,7 +870,9 @@ static double linesearch(lb_ctx *c, const double *xk, const double *pk, double a
   vaxpy(xp, pk, -2.0 * step, m);
   p02 = lb_cost(c, xp);
   gphi_0 = (p01 - p02) / (2.0 * step);
+  const double n0 = diff_noise(p01, p02, step);
   mu = (tol - phi_0) / (rho * gphi_0);
+  const double nmu = fabs(mu) * (n0 / fabs(gphi_0) + cost_noise(tol, phi_0) / fabs(tol - phi_0));
   if (!isnormal(mu)) {
     free(xp);
     return mu;
@@ -845,12 +885,18 @@ static double linesearch(lb_ctx *c, const double *xk, const double *pk, double a
     memcpy(xp, xk, sizeof(double) * m);
     vaxpy(xp, pk, alphai, m);
     phi_alphai = lb_cost(c, xp);
+    lb_decide(c, phi_alphai, tol, cost_noise(phi_alphai, tol));
     if (phi_alphai < tol) {
       alphak = alphai;
       break;
     }
+    lb_decide(c, phi_alphai, phi_0 + alphai * gphi_0,
+              cost_noise(phi_alphai, phi_0) + fabs(alphai) * n0);
+    if (!(phi_alphai > phi_0 + alphai * gphi_0) && ci > 1)
+      lb_decide(c, phi_alphai, phi_alphai1, cost_noise(phi_alphai, phi_alphai1));
     if ((phi_alphai > phi_0 + alphai * gphi_0) || (ci > 1 && phi_alphai >= phi_alphai1)) {
-      alphak = ls_zoom(c, xk, pk, alphai1, alphai, xp, phi_0, gphi_0, sigma, rho, t2, t3, m, step);
+      alphak = ls_zoom(c, xk, pk, alphai1, alphai, xp, phi_0, gphi_0, n0, sigma, rho, t2, t3, m,
+                       step);
       break;
     }
     vaxpy(xp, pk, step, m);
@@ -858,14 +904,19 @@ static double linesearch(lb_ctx *c, const double *xk, const double *pk, double a
     vaxpy(xp, pk, -2.0 * step, m);
     p02 = lb_cost(c, xp);
     gphi_i = (p01 - p02) / (2.0 * step);
+    const double ni = diff_noise(p01, p02, step);
+    lb_decide(c, fabs(gphi_i), -sigma * gphi_0, ni + sigma * n0);
     if (fabs(gphi_i) <= -sigma * gphi_0) {
       alphak = alphai;
       break;
     }
+    lb_decide(c, gphi_i, 0.0, ni);
     if (gphi_i >= 0) {
-      alphak = ls_zoom(c, xk, pk, alphai, alphai1, xp, phi_0, gphi_0, sigma, rho, t2, t3, m, step);
+      alphak = ls_zoom(c, xk, pk, alphai, alphai1, xp, phi_0, gphi_0, n0, sigma, rho, t2, t3, m,
+                       step);
       break;
     }
+    lb_decide(c, mu, 2.0 * alphai - alphai1, nmu);
     if (mu <= (2.0 * alphai - alphai1)) {
       alphai1 = alphai;
       alphai = mu;
@@ -882,10 +933,14 @@ static double linesearch(lb_ctx *c, const double *xk, const double *pk, double a
   return alphak;
 }
 
-void orc_lbfgs(const orc_problem *P, double *pp, const double *x, int itmax, int M, int robust,
-               double nu) {
+static double g_lbfgs_margin = HUGE_VAL;
+double orc_lbfgs_last_margin(void) { return g_lbfgs_margin; }
+
+void orc_lbfgs_traced(const orc_problem *P, double *pp, const double *x, int itmax, int M,
+                      int robust, double nu, orc_lbfgs_trace *tr) {
   const int m = 8 * P->N * P->Mt;
-  lb_ctx ctx = {P, x, robust, nu};
+  lb_ctx ctx = {P, x, robust, nu, 0, HUGE_VAL};
+  if (tr) tr->niter = 0;
   if (M < 1) M = 1;
   double *gk = (double *)xcalloc(m, sizeof(double)), *xk1 = (double *)xcalloc(m, sizeof(double));
   double *xk = (double *)xcalloc(m, sizeof(double)), *pk = (double *)xcalloc(m, sizeof(double));
@@ -907,7 +962,8 @@ void orc_lbfgs(const orc_problem *P, double *pp, const double *x, int itmax, int
     step = (t > 1e-9) ? t : 1e-9;
   }
   while (ck < itmax && isnormal(gradnrm) && gradnrm > 1e-17) {
-    mult_hessian(m, pk, gk, s, y, rho, ck < M ? ck : M, ci);
+    const long long ncost0 = ctx.ncost;
+    orc_mult_hessian(m, pk, gk, s, y, rho, ck < M ? ck : M, ci);
     for (int i = 0; i < m; i++) pk[i] = -pk[i];
     double alphak = linesearch(&ctx, xk, pk, 10.0, 0.1, 0.01, 9, 0.1, 0.5, m, step);
     if (!isnormal(alphak) || fabs(alphak) < 1e-12) break;
@@ -922,6 +978,14 @@ void orc_lbfgs(const orc_problem *P, double *pp, const double *x, int itmax, int
     vaxpy(y + cm, gk, 1.0, m);
     rho[ci] = 1.0 / vdot(y + cm, s + cm, m);
     memcpy(xk, xk1, sizeof(double) * m);
+    if (tr) {
+      tr->alphak[ck] = alphak;
+      tr->ncost[ck] = ctx.ncost - ncost0;
+      tr->slot[ck] = ci;
+      tr->gnorm[ck] = gradnrm;
+      memcpy(tr->iterates + (size_t)m * ck, xk, sizeof(double) * m);
+      tr->niter = ck + 1;
+    }
     ck++;
     if (cm < (M - 1) * m) {
       cm += m;
@@ -932,6 +996,13 @@ void orc_lbfgs(const orc_problem *P, double *pp, const double *x, int itmax, int
   }
   memcpy(pp, xk, sizeof(double) * m);
   free(gk); free(xk1); free(xk); free(pk); free(s); free(y); free(rho);
+  g_lbfgs_margin = ctx.margin;
+  if (tr) tr->margin = ctx.margin;
+}
+
+void orc_lbfgs(const orc_problem *P, double *pp, const double *x, int itmax, int M, int robust,
+               double nu) {
+  orc_lbfgs_traced(P, pp, x, itmax, M, robust, nu, NULL);
 }
 
 /* ---- RTR / RSD / NSD: the per-row evaluators (Dirac/rtr_solve.c, Dirac/rtr_solve_robust.c) -------

@@ -48,6 +48,26 @@ double orc_update_w_and_nu(double nu0, double *w, const double *ed, int n, doubl
 long orc_noise_decisions(int reset);
 void orc_lbfgs(const orc_problem *P, double *pp, const double *x, int itmax, int M, int robust,
                double nu);
+/* the two-loop recursion (lbfgs.c:33-111): pk = H g from M valid pairs, ii the slot written next */
+void orc_mult_hessian(int m, double *pk, const double *gk, const double *s, const double *y,
+                      const double *rho, int M, int ii);
+/* what one LBFGS run did: per iteration k the accepted step, the cost evaluations of its line
+ * search, the history slot written, ||g|| after the update and the iterate (m doubles); arrays of
+ * itmax entries.  margin: the smallest margin of the line search's decisions over the run, in units
+ * of the rounding noise of the costs behind them (see lb_decide) */
+typedef struct {
+  double *alphak;
+  long long *ncost;
+  int *slot;
+  double *gnorm;
+  double *iterates;
+  int niter;
+  double margin;
+} orc_lbfgs_trace;
+void orc_lbfgs_traced(const orc_problem *P, double *pp, const double *x, int itmax, int M,
+                      int robust, double nu, orc_lbfgs_trace *tr);
+/* margin (as in orc_lbfgs_trace) of the last LBFGS run, traced or not; HUGE_VAL before any */
+double orc_lbfgs_last_margin(void);
 /* RTR / RSD / NSD (solver_mode 4-6): per-row evaluators; the solver of one chunk is supplied by
  * oracle/rtr_harness.cpp (the control flow of rtr_algo.h on these evaluators) */
 double orc_rtr_raw(const orc_problem *P, int k, int t0, int ntiles, const double *y,

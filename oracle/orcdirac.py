@@ -31,6 +31,22 @@ class orc_sky(C.Structure):
                                   "spec_idx2")]
 
 
+class orc_lbfgs_trace(C.Structure):
+    _fields_ = [("alphak", dp), ("ncost", C.POINTER(C.c_longlong)), ("slot", ip), ("gnorm", dp),
+                ("iterates", dp), ("niter", C.c_int), ("margin", C.c_double)]
+
+
+def mult_hessian(g, s, y, rho, npairs, next_):
+    """orc_mult_hessian: H g of the two-loop recursion (without the sign of the search direction)
+    from s, y [Mmem, m], rho [Mmem], `npairs` valid pairs and `next_` the slot written next"""
+    L = C.CDLL(ORC_PATH)
+    L.orc_mult_hessian.argtypes = [C.c_int, dp, dp, dp, dp, dp, C.c_int, C.c_int]
+    g, s, y, rho = (np.ascontiguousarray(a, dtype=np.float64) for a in (g, s, y, rho))
+    pk = np.zeros(len(g))
+    L.orc_mult_hessian(len(g), _d(pk), _d(g), _d(s), _d(y), _d(rho), npairs, next_)
+    return pk
+
+
 def available():
     return os.path.exists(ORC_PATH)
 
@@ -66,6 +82,11 @@ class Oracle:
         L.orc_update_w_and_nu.restype = d
         L.orc_update_w_and_nu.argtypes = [d, dp, dp, i, d, d]
         L.orc_lbfgs.argtypes = [pp, dp, dp, i, i, i, d]
+        L.orc_mult_hessian.argtypes = [i, dp, dp, dp, dp, dp, i, i]
+        L.orc_lbfgs_traced.argtypes = [pp, dp, dp, i, i, i, d, C.POINTER(orc_lbfgs_trace)]
+        L.orc_lbfgs_last_margin.restype = d
+        L.orc_noise_decisions.restype = C.c_long
+        L.orc_noise_decisions.argtypes = [i]
         L.orc_sagefit.restype = i
         L.orc_sagefit.argtypes = [pp, dp, dp, i, i, i, i, i, i, d, d, dp, dp, dp]
         L.orc_bfgsfit.restype = i
@@ -246,6 +267,23 @@ class Oracle:
                                 lbfgs_m, linsolv, solver_mode, nulow, nuhigh, C.byref(nu),
                                 C.byref(r0), C.byref(r1))
         return rv, nu.value, r0.value, r1.value
+
+    def lbfgs_trace(self, x, pp, itmax, M, robust=False, nu=2.0):
+        """orc_lbfgs with its trace.  returns dict(p [final], niter, alphak, ncost, slot, gnorm
+        [per iteration], iterates [niter, m], margin [smallest line-search decision margin])"""
+        p = np.array(pp, dtype=np.float64)
+        n = max(itmax, 1)
+        alphak, gnorm = np.zeros(n), np.zeros(n)
+        ncost = np.zeros(n, dtype=np.int64)
+        slot = np.zeros(n, dtype=np.int32)
+        it = np.zeros((n, self.m))
+        tr = orc_lbfgs_trace(_d(alphak), ncost.ctypes.data_as(C.POINTER(C.c_longlong)),
+                             slot.ctypes.data_as(ip), _d(gnorm), _d(it.reshape(-1)), 0, 0.0)
+        self.L.orc_lbfgs_traced(C.byref(self.P), _d(p), _d(np.ascontiguousarray(x)), itmax, M,
+                                int(robust), nu, C.byref(tr))
+        k = tr.niter
+        return dict(p=p, niter=k, alphak=alphak[:k], ncost=ncost[:k], slot=slot[:k],
+                    gnorm=gnorm[:k], iterates=it[:k], margin=tr.margin)
 
     def bfgsfit(self, x, pp, max_lbfgs=10, lbfgs_m=7, solver_mode=1, mean_nu=2.0, **_ignored):
         r0, r1 = C.c_double(0), C.c_double(0)

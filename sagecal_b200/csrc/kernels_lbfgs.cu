@@ -5,7 +5,9 @@
 // of one thread-block cluster: each of the 8 CTAs owns a slice of every vector, a dot product is a
 // CTA reduction followed by an exchange of the 8 partial sums through distributed shared memory, and
 // the 2M+1 dependent dot products / 2M axpys run back to back without touching the host.  No scalar
-// ever leaves the device: rho_j lives in a device array, written by k_lbfgs_update.
+// ever leaves the device: rho_j lives in a device array, written by k_lbfgs_update.  The alpha_i of
+// one recursion sit in dynamic shared memory, one double per pair, so the memory size has no cap
+// below what one CTA can hold (db_lbfgs_direction_max_pairs: ~29000 pairs on an H100).
 #include <cooperative_groups.h>
 
 #include "internal.cuh"
@@ -46,7 +48,7 @@ struct LbfgsDirArgs {
 __global__ void __cluster_dims__(LB_CTAS, 1, 1) __launch_bounds__(LB_THREADS)
 k_lbfgs_direction(LbfgsDirArgs a) {
   __shared__ double red[16 + 8];
-  __shared__ double alphai[64];
+  extern __shared__ double alphai[];  // [npairs]
   cg::cluster_group cl = cg::this_cluster();
   const int rank = (int)cl.block_rank();
   const int per = (a.m + LB_CTAS - 1) / LB_CTAS;
@@ -149,11 +151,29 @@ k_lbfgs_update(const double *__restrict__ gk, const double *__restrict__ sk, dou
 }
 
 extern "C" {
+// the most pairs k_lbfgs_direction can hold: the opt-in shared memory of one CTA less its static part
+int db_lbfgs_direction_max_pairs(void) {
+  static int maxp = -1;
+  if (maxp < 0) {
+    int dev, optin;
+    cudaFuncAttributes fa;
+    DB_CHECK(cudaGetDevice(&dev));
+    DB_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    DB_CHECK(cudaFuncGetAttributes(&fa, k_lbfgs_direction));
+    maxp = (int)((optin - (long long)fa.sharedSizeBytes) / (long long)sizeof(double));
+  }
+  return maxp;
+}
+// npairs <= db_lbfgs_direction_max_pairs() (the caller checks)
 void db_launch_lbfgs_direction(double *pk, const double *gk, const double *s, const double *y,
                                const double *rho, int m, int npairs, int next, cudaStream_t st) {
   LbfgsDirArgs a;
   a.pk = pk; a.gk = gk; a.s = s; a.y = y; a.rho = rho; a.m = m; a.npairs = npairs; a.next = next;
-  k_lbfgs_direction<<<LB_CTAS, LB_THREADS, 0, st>>>(a);
+  const size_t smem = sizeof(double) * (size_t)npairs;
+  if (smem > 48 * 1024)
+    DB_CHECK(cudaFuncSetAttribute(k_lbfgs_direction, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)smem));
+  k_lbfgs_direction<<<LB_CTAS, LB_THREADS, smem, st>>>(a);
 }
 void db_launch_lbfgs_nrm2(const double *g, int m, double *out, cudaStream_t st) {
   k_lbfgs_nrm2<<<LB_CTAS, LB_THREADS, 0, st>>>(g, m, out);

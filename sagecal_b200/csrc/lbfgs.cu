@@ -26,6 +26,7 @@
 #include "problem.h"
 
 extern "C" {
+int db_lbfgs_direction_max_pairs(void);
 void db_launch_lbfgs_direction(double *pk, const double *gk, const double *s, const double *y,
                                const double *rho, int m, int npairs, int next, cudaStream_t st);
 void db_launch_lbfgs_nrm2(const double *g, int m, double *out, cudaStream_t st);
@@ -307,10 +308,22 @@ static double linesearch(LbfgsCtx *c, double alpha1, double sigma, double rho, d
   return alphak;
 }
 
+// What one run of the iteration did, for the tests (dirac_b200_lbfgs_trace); per iteration k:
+// the accepted step, the cost evaluations of its line search, the history slot it wrote, ||g|| after
+// the update and the iterate after it (m doubles).  Arrays of at least itmax entries.
+struct LbfgsTrace {
+  double *alphak;
+  long long *ncost;
+  int *slot;
+  double *gnorm;
+  double *iterates;
+  int niter;
+};
+
 // p: m x 1 in/out (host).  robust != 0 -> Student's-t cost with nu.
 // Iteration logic of lbfgs_fit_fullbatch (lbfgs.c:479-640); vectors on the device.
-void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
-                  double nu) {
+static void lbfgs_run(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
+                      double nu, LbfgsTrace *tr) {
   DevProblem &d = pr->d;
   LbfgsCtx ctx;
   ctx.pr = pr;
@@ -318,8 +331,14 @@ void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, in
   ctx.nu = nu;
   ctx.m = m;
   ctx.ncost = ctx.ngrad = 0;
+  if (tr) tr->niter = 0;
   if (M < 1) M = 1;
-  if (M > 64) M = 64;  // k_lbfgs_direction keeps the alpha_i of one recursion in shared memory
+  if (M > db_lbfgs_direction_max_pairs()) {
+    // the alpha_i of one recursion live in the shared memory of k_lbfgs_direction
+    fprintf(stderr, "dirac_b200: LBFGS memory size %d exceeds the %d pairs the two-loop recursion "
+                    "can hold; the LBFGS stage is skipped\n", M, db_lbfgs_direction_max_pairs());
+    return;
+  }
   // one allocation: xk | xk1 | gk | pk | s[M] | y[M] | rho[M]
   double *ws = (double *)db_malloc(sizeof(double) * ((size_t)m * (4 + 2 * (size_t)M) + M + 8));
   double *xk = ws, *xk1 = xk + m, *gk = xk1 + m, *pk = gk + m, *s = pk + m,
@@ -345,6 +364,7 @@ void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, in
   cm = 0;
   ci = 0;
   while (ck < itmax && isnormal(gradnrm) && gradnrm > STOP) {
+    const long long ncost0 = ctx.ncost;
     db_launch_lbfgs_direction(pk, gk, s, y, rho, m, ck < M ? ck : M, ci, d.stream);
     db_count_launch(1);
     line_setup(&ctx, xk, pk);
@@ -357,6 +377,15 @@ void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, in
     db_launch_lbfgs_update(gk, sk, yk, xk1, xk, m, rho + ci, nrm_dev, d.stream);
     db_count_launch(2);
     gradnrm = sqrt(db_read_scalar(pr, 24));
+    if (tr) {
+      tr->alphak[ck] = alphak;
+      tr->ncost[ck] = ctx.ncost - ncost0;
+      tr->slot[ck] = ci;
+      tr->gnorm[ck] = gradnrm;
+      DB_CHECK(cudaMemcpy(tr->iterates + (size_t)m * ck, xk, sizeof(double) * m,
+                          cudaMemcpyDeviceToHost));
+      tr->niter = ck + 1;
+    }
     ck++;
     if (cm < (M - 1) * m) {
       cm += m;
@@ -368,6 +397,11 @@ void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, in
   DB_CHECK(cudaMemcpyAsync(p, xk, sizeof(double) * m, cudaMemcpyDeviceToHost, d.stream));
   db_stream_sync(d.stream);
   db_free(ws);
+}
+
+void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
+                  double nu) {
+  lbfgs_run(pr, p, m, itmax, M, robust, nu, nullptr);
 }
 
 // test hook: the line model of the resident problem along pk from xk (host vectors of npar doubles),
@@ -405,4 +439,84 @@ extern "C" void dirac_b200_line_model(dirac_b200_problem *pr, const double *xk, 
   db_download_vis(pr, pr->res, res);
   DB_CHECK(cudaGetLastError());
   db_free(dx);
+}
+
+// test hook: LBFGS on the resident problem's data from p (host, npar doubles, in/out) as bfgsfit runs
+// it, with the trace of every iteration (LbfgsTrace; arrays of itmax entries, iterates itmax x npar).
+// Returns the number of iterations, or -1 if the memory size M cannot be held.
+extern "C" int dirac_b200_lbfgs_trace(dirac_b200_problem *pr, double *p, int itmax, int M, int robust,
+                                      double nu, double *alphak, long long *ncost, int *slot,
+                                      double *gnorm, double *iterates) {
+  if ((M < 1 ? 1 : M) > db_lbfgs_direction_max_pairs()) return -1;
+  LbfgsTrace tr;
+  tr.alphak = alphak; tr.ncost = ncost; tr.slot = slot; tr.gnorm = gnorm; tr.iterates = iterates;
+  lbfgs_run(pr, p, (int)pr->d.npar, itmax, M, robust, nu, &tr);
+  return tr.niter;
+}
+
+// test hook: one two-loop recursion (k_lbfgs_direction) on host vectors exactly as db_lbfgs_fit
+// launches it: g [m], s and y [Mmem][m], rho [Mmem]; pk [m] out.  Returns -1 without launching if
+// npairs > Mmem, next >= Mmem or the kernel cannot hold npairs.
+extern "C" int dirac_b200_lbfgs_direction(int m, int Mmem, int npairs, int next, const double *g,
+                                          const double *s, const double *y, const double *rho,
+                                          double *pk) {
+  if (m < 1 || Mmem < 1 || npairs < 0 || npairs > Mmem || next < 0 || next >= Mmem ||
+      npairs > db_lbfgs_direction_max_pairs())
+    return -1;
+  const size_t nv = (size_t)m * (2 + 2 * (size_t)Mmem) + Mmem;
+  double *w = (double *)db_malloc(sizeof(double) * nv);
+  double *dg = w, *dpk = dg + m, *ds = dpk + m, *dy = ds + (size_t)m * Mmem,
+         *drho = dy + (size_t)m * Mmem;
+  DB_CHECK(cudaMemcpy(dg, g, sizeof(double) * m, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(ds, s, sizeof(double) * m * Mmem, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(dy, y, sizeof(double) * m * Mmem, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(drho, rho, sizeof(double) * Mmem, cudaMemcpyHostToDevice));
+  db_launch_lbfgs_direction(dpk, dg, ds, dy, drho, m, npairs, next, 0);
+  DB_CHECK(cudaGetLastError());
+  DB_CHECK(cudaMemcpy(pk, dpk, sizeof(double) * m, cudaMemcpyDeviceToHost));
+  db_free(w);
+  return 0;
+}
+
+// test hook: k_lbfgs_step then k_lbfgs_update as one iteration of db_lbfgs_fit runs them, with the
+// pair written into slot ci of a rho[Mmem] array (rho_in host, copied).  Out (host): xk1, sk, yk [m],
+// rho [Mmem], ||gk_new||^2 in gg[0], and xk after the update in xk_out [m].
+extern "C" int dirac_b200_lbfgs_step_update(int m, double alpha, const double *xk, const double *pk,
+                                            const double *gk_old, const double *gk_new, int Mmem,
+                                            int ci, const double *rho_in, double *xk1, double *sk,
+                                            double *yk, double *rho, double *gg, double *xk_out) {
+  if (m < 1 || Mmem < 1 || ci < 0 || ci >= Mmem) return -1;
+  const size_t nv = (size_t)m * 7 + Mmem + 1;
+  double *w = (double *)db_malloc(sizeof(double) * nv);
+  double *dx = w, *dp = dx + m, *dg0 = dp + m, *dg1 = dg0 + m, *dx1 = dg1 + m, *ds = dx1 + m,
+         *dy = ds + m, *drho = dy + m, *dgg = drho + Mmem;
+  DB_CHECK(cudaMemcpy(dx, xk, sizeof(double) * m, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(dp, pk, sizeof(double) * m, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(dg0, gk_old, sizeof(double) * m, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(dg1, gk_new, sizeof(double) * m, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(drho, rho_in, sizeof(double) * Mmem, cudaMemcpyHostToDevice));
+  db_launch_lbfgs_step(dx, dp, dg0, dx1, ds, dy, m, alpha, 0);
+  DB_CHECK(cudaGetLastError());
+  DB_CHECK(cudaMemcpy(xk1, dx1, sizeof(double) * m, cudaMemcpyDeviceToHost));
+  DB_CHECK(cudaMemcpy(sk, ds, sizeof(double) * m, cudaMemcpyDeviceToHost));
+  db_launch_lbfgs_update(dg1, ds, dy, dx1, dx, m, drho + ci, dgg, 0);
+  DB_CHECK(cudaGetLastError());
+  DB_CHECK(cudaMemcpy(yk, dy, sizeof(double) * m, cudaMemcpyDeviceToHost));
+  DB_CHECK(cudaMemcpy(rho, drho, sizeof(double) * Mmem, cudaMemcpyDeviceToHost));
+  DB_CHECK(cudaMemcpy(gg, dgg, sizeof(double), cudaMemcpyDeviceToHost));
+  DB_CHECK(cudaMemcpy(xk_out, dx, sizeof(double) * m, cudaMemcpyDeviceToHost));
+  db_free(w);
+  return 0;
+}
+
+// test hook: ||g||^2 of k_lbfgs_nrm2 for a host vector g [m]
+extern "C" double dirac_b200_lbfgs_nrm2(int m, const double *g) {
+  double *w = (double *)db_malloc(sizeof(double) * ((size_t)m + 1));
+  double out;
+  DB_CHECK(cudaMemcpy(w, g, sizeof(double) * m, cudaMemcpyHostToDevice));
+  db_launch_lbfgs_nrm2(w, m, w + m, 0);
+  DB_CHECK(cudaGetLastError());
+  DB_CHECK(cudaMemcpy(&out, w + m, sizeof(double), cudaMemcpyDeviceToHost));
+  db_free(w);
+  return out;
 }

@@ -102,6 +102,50 @@ class DiracB200(DiracAPI):
     def launch_count(self) -> int:
         return int(self.lib.dirac_b200_launch_count())
 
+    def lbfgs_direction(self, g, s, y, rho, npairs, next_):
+        """one two-loop recursion of k_lbfgs_direction (dirac_b200_lbfgs_direction) on host vectors:
+        g [m], s and y [Mmem, m], rho [Mmem], `npairs` valid pairs, `next_` the slot written next.
+        returns pk = -H g [m], or None where the hook refuses the arguments"""
+        L = self.lib
+        L.dirac_b200_lbfgs_direction.restype = C.c_int
+        L.dirac_b200_lbfgs_direction.argtypes = [C.c_int] * 4 + [c_double_p] * 5
+        g = np.ascontiguousarray(g, dtype=np.float64)
+        s = np.ascontiguousarray(s, dtype=np.float64)
+        y = np.ascontiguousarray(y, dtype=np.float64)
+        rho = np.ascontiguousarray(rho, dtype=np.float64)
+        Mmem, m = s.shape
+        assert y.shape == s.shape and g.shape == (m,) and rho.shape == (Mmem,)
+        pk = np.zeros(m)
+        rv = L.dirac_b200_lbfgs_direction(m, Mmem, npairs, next_, dptr(g), dptr(s), dptr(y),
+                                          dptr(rho), dptr(pk))
+        return None if rv != 0 else pk
+
+    def lbfgs_step_update(self, alpha, xk, pk, gk_old, gk_new, rho, ci):
+        """k_lbfgs_step then k_lbfgs_update into slot ci of rho (dirac_b200_lbfgs_step_update).
+        returns dict(xk1, sk, yk, rho, gg = ||gk_new||^2, xk = xk after the update)"""
+        L = self.lib
+        L.dirac_b200_lbfgs_step_update.restype = C.c_int
+        L.dirac_b200_lbfgs_step_update.argtypes = ([C.c_int, C.c_double] + [c_double_p] * 4
+                                                   + [C.c_int, C.c_int] + [c_double_p] * 7)
+        a = [np.ascontiguousarray(v, dtype=np.float64) for v in (xk, pk, gk_old, gk_new, rho)]
+        m, Mmem = len(a[0]), len(a[4])
+        out = dict(xk1=np.zeros(m), sk=np.zeros(m), yk=np.zeros(m), rho=np.zeros(Mmem),
+                   gg=np.zeros(1), xk=np.zeros(m))
+        rv = L.dirac_b200_lbfgs_step_update(m, alpha, *[dptr(v) for v in a[:4]], Mmem, ci,
+                                            dptr(a[4]), *[dptr(out[k]) for k in
+                                                          ("xk1", "sk", "yk", "rho", "gg", "xk")])
+        assert rv == 0
+        out["gg"] = float(out["gg"][0])
+        return out
+
+    def lbfgs_nrm2(self, g):
+        """||g||^2 of k_lbfgs_nrm2 (dirac_b200_lbfgs_nrm2)"""
+        L = self.lib
+        L.dirac_b200_lbfgs_nrm2.restype = C.c_double
+        L.dirac_b200_lbfgs_nrm2.argtypes = [C.c_int, c_double_p]
+        g = np.ascontiguousarray(g, dtype=np.float64)
+        return float(L.dirac_b200_lbfgs_nrm2(len(g), dptr(g)))
+
     def kernel_count(self, kind) -> int:
         return int(self.lib.dirac_b200_kernel_count(kind))
 
@@ -207,6 +251,30 @@ class DeviceProblem:
 
     #: operation bits of one rtr_eval evaluation (rtr.cu: RTR_HOOK_*)
     RTR_COST, RTR_VEC, RTR_COUNTS, RTR_ETA, RTR_UNIT = 1, 2, 4, 8, 16
+
+    def lbfgs_trace(self, pp, itmax, M, robust=False, nu=2.0):
+        """LBFGS on the resident data from pp as bfgsfit runs it, traced (dirac_b200_lbfgs_trace).
+        returns dict(p [final], niter, alphak, ncost, slot, gnorm [per iteration], iterates
+        [niter, m]), or None where the memory size M cannot be held"""
+        L = self.api.lib
+        L.dirac_b200_lbfgs_trace.restype = C.c_int
+        L.dirac_b200_lbfgs_trace.argtypes = [C.c_void_p, c_double_p, C.c_int, C.c_int, C.c_int,
+                                             C.c_double, c_double_p, C.POINTER(C.c_longlong),
+                                             C.POINTER(C.c_int), c_double_p, c_double_p]
+        p = np.array(pp, dtype=np.float64)
+        n = max(itmax, 1)
+        alphak, gnorm = np.zeros(n), np.zeros(n)
+        ncost = np.zeros(n, dtype=np.int64)
+        slot = np.zeros(n, dtype=np.int32)
+        it = np.zeros((n, self.m))
+        k = L.dirac_b200_lbfgs_trace(self.h, dptr(p), itmax, M, int(robust), nu, dptr(alphak),
+                                     ncost.ctypes.data_as(C.POINTER(C.c_longlong)),
+                                     slot.ctypes.data_as(C.POINTER(C.c_int)), dptr(gnorm),
+                                     dptr(it.reshape(-1)))
+        if k < 0:
+            return None
+        return dict(p=p, niter=k, alphak=alphak[:k], ncost=ncost[:k], slot=slot[:k],
+                    gnorm=gnorm[:k], iterates=it[:k])
 
     def rtr_eval(self, k, ck, evals, xw=None, nu=2.0, keep=True, force_device=False):
         """the RTR device evaluator of cluster k, chunk ck on the data vector as hidden data

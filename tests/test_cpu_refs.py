@@ -1,11 +1,12 @@
-"""CPU: the plain references the GPU tests of the line model and of the segmented sky staging lean
-on, pinned against the restatement (oracle/liboracle.so) before a GPU is involved."""
+"""CPU: the plain references the GPU tests of the line model, the RTR evaluator, the IRLS update, the
+LBFGS two-loop recursion and the segmented sky staging lean on, pinned against the restatement
+(oracle/liboracle.so) before a GPU is involved."""
 import numpy as np
 import pytest
 
 import orcdirac
-from util import (big_cluster_sky, irls_ref, line_model_ref, relerr, rtr_eval_ref, rtr_weights_ref,
-                  small_problem, split_cluster)
+from util import (big_cluster_sky, irls_ref, lbfgs_pairs, line_model_ref, mult_hessian_ref, relerr,
+                  rtr_eval_ref, rtr_weights_ref, small_problem, split_cluster)
 
 needs_oracle = pytest.mark.skipif(not orcdirac.available(), reason="oracle/liboracle.so not built")
 
@@ -148,3 +149,25 @@ def test_sky_split_identity_on_the_oracle():
     xb = orcdirac.OracleSky(split_cluster(big, parts)).predict_multifreq(u, v, w, freqs, 6e5, 1,
                                                                          np.zeros(8 * R * 3))
     assert relerr(xb, xa) < 1e-13
+
+
+@needs_oracle
+@pytest.mark.parametrize("M", [1, 2, 7, 65, 100])
+def test_mult_hessian_reference_matches_oracle(M):
+    """util.mult_hessian_ref against orc_mult_hessian (the reference's mult_hessian restated in C) in
+    every state the LBFGS driver produces: the partial histories (npairs, next) = (k, k), k < M, and
+    the full history at every next slot; one pair with y . s < 0 (the reference keeps it)"""
+    m = 37 if M > 7 else 53
+    g, s, y, rho = lbfgs_pairs(m, M, seed=M, negative=M // 2)
+    assert rho[M // 2] < 0
+    states = [(k, k) for k in range(M)] + [(M, j) for j in range(M)]
+    for npairs, nxt in states:
+        want = orcdirac.mult_hessian(g, s, y, rho, npairs, nxt)
+        got, scale = mult_hessian_ref(g, s, y, rho, npairs, nxt)
+        if npairs == 0:
+            assert np.array_equal(got, g) and np.array_equal(want, g)
+            continue
+        assert (np.abs(got - want) <= 1e-14 * scale).all(), (npairs, nxt,
+                                                                np.max(np.abs(got - want) / scale))
+        # the pairs matter: the answer is far from the scaled gradient of a memoryless step
+        assert relerr(g * (s[0] @ y[0]) / (y[0] @ y[0]), got) > 1e-3

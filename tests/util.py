@@ -271,3 +271,84 @@ def relerr(a, b):
         assert keep.any(), "no reference value to compare with"
         a, b = np.broadcast_to(a, b.shape)[keep], b[keep]
     return float(np.max(np.abs(a - b)) / (np.max(np.abs(b)) + 1e-300))
+
+
+def mult_hessian_ref(g, s, y, rho, npairs, next_):
+    """the two-loop recursion of the reference (mult_hessian, lbfgs.c:33-111) restated literally:
+    the same `idx` order of the ring buffer (oldest ... newest pair), the same gamma from the newest
+    pair; dot products summed in long double.  s, y [Mmem, m], rho [Mmem]; `npairs` valid pairs,
+    `next_` the slot written next.  returns (H g, magnitude companion): the companion is the same
+    recursion on absolute values, the scale of the rounding error of any summation order"""
+    g = np.asarray(g, dtype=np.float64)
+    s = np.asarray(s, dtype=np.float64)
+    y = np.asarray(y, dtype=np.float64)
+    rho = np.asarray(rho, dtype=np.float64)
+    M = npairs
+    idx = np.zeros(M, dtype=int)
+    if M > 0:
+        ii = next_ - 1 if next_ > 0 else M - 1
+        for ci in range(M - ii - 1):
+            idx[ci] = ii + ci + 1
+        for ci in range(M - ii - 1, M):
+            idx[ci] = ci - M + ii + 1
+    dot = lambda a, b: lsum(a * np.asarray(b, dtype=np.longdouble))
+    pk, pa = g.copy(), np.abs(g)
+    alphai, alpha_a = np.zeros(M), np.zeros(M)
+    for ci in range(M):
+        j = idx[M - ci - 1]
+        alphai[M - ci - 1] = rho[j] * dot(s[j], pk)
+        alpha_a[M - ci - 1] = abs(rho[j]) * dot(np.abs(s[j]), pa)
+        pk = pk - alphai[M - ci - 1] * y[j]
+        pa = pa + alpha_a[M - ci - 1] * np.abs(y[j])
+    if M > 0:
+        j = idx[M - 1]
+        gamma = dot(s[j], y[j]) / dot(y[j], y[j])
+        pk = pk * gamma
+        pa = pa * (dot(np.abs(s[j]), np.abs(y[j])) / dot(y[j], y[j]))
+    for ci in range(M):
+        j = idx[ci]
+        beta = rho[j] * dot(y[j], pk)
+        beta_a = abs(rho[j]) * dot(np.abs(y[j]), pa)
+        pk = pk + (alphai[ci] - beta) * s[j]
+        pa = pa + (alpha_a[ci] + beta_a) * np.abs(s[j])
+    return pk, pa
+
+
+def lbfgs_pairs(m, Mmem, seed, cond=1e3, noise=1e-3, negative=None):
+    """an LBFGS history of Mmem pairs of length m as a curvature model produces them: y = B s + noise
+    with B SPD of condition ~cond (diagonal, a log-spaced spectrum in random order), rho = 1 / (y . s).  `negative`: the slot of one pair with y . s < 0
+    (y flipped).  returns (g, s [Mmem, m], y [Mmem, m], rho [Mmem])"""
+    rng = np.random.default_rng(seed)
+    lam = np.exp(np.linspace(0.0, np.log(cond), m))[rng.permutation(m)]
+    s = rng.normal(0, 1, (Mmem, m)) * rng.uniform(0.1, 2.0, (Mmem, 1))
+    y = s * lam + noise * rng.normal(0, 1, (Mmem, m)) * np.sqrt(lam)
+    if negative is not None:
+        y[negative] = -y[negative]
+    rho = 1.0 / np.einsum("ij,ij->i", y, s)
+    g = rng.normal(0, 1, m)
+    return g, s, y, rho
+
+
+#: LBFGS runs traced iteration by iteration (tests/test_gpu_lbfgs.py) and checked against the compiled
+#: reference (tests/test_oracle_vs_ref.py): (id, problem, lbfgs_m, max_lbfgs, robust).  Every run starts
+#: from pp0 + 0.1 N(0, 1) (lbfgs_start) so that the search directions matter; max_lbfgs >= 2 lbfgs_m + 2
+#: wraps the history at least twice.  Seeds are those whose line-search decisions all lie far above
+#: rounding level (orc_lbfgs_traced's margin; the Gaussian product evaluates its costs from the quartic
+#: of the line model, the restatement directly).  robust-m80 runs 66 iterations with 80 pairs: past
+#: the 64 pairs k_lbfgs_direction once held.
+LBFGS_TRACE_CASES = [
+    ("gauss-plain-m1", dict(N=8, M=2, tilesz=8, seed=1), 1, 6, False),
+    ("gauss-hybrid-m3", dict(N=8, M=3, tilesz=8, nchunk=[1, 2, 3], seed=1), 3, 10, False),
+    ("gauss-plain-m7", dict(N=8, M=3, tilesz=8, kmean=1.0, seed=2), 7, 18, False),
+    ("robust-plain-m3", dict(N=8, M=2, tilesz=8, outliers=0.02, seed=1), 3, 10, True),
+    ("robust-hybrid-m7", dict(N=8, M=3, tilesz=8, nchunk=[2, 1, 3], outliers=0.02, seed=2), 7, 16,
+     True),
+    ("robust-m80", dict(N=20, M=8, tilesz=3, kmean=1.0, seed=4), 80, 66, True),
+]
+LBFGS_TRACE_NU = 4.0
+
+
+def lbfgs_start(pr, seed):
+    """the perturbed starting Jones of an LBFGS_TRACE_CASES run on the problem of that seed"""
+    rng = np.random.default_rng(seed + 100)
+    return pr.pp0 + 0.1 * rng.normal(0, 1, pr.pp0.shape)
