@@ -193,6 +193,16 @@ double dirac_b200_predict(dirac_b200_problem *pr, const double *pp, double *out,
 /* LBFGS gradient in the reference's sign convention (func_grad / func_grad_robust,
  * robust_lbfgs.c:569-669,322-416); g has 8*N*Mt doubles. */
 void dirac_b200_grad(dirac_b200_problem *pr, const double *pp, double *g, int robust, double nu);
+/* Student's-t cost sum log(1+e^2/nu) over the rows [row0, row0+nrows) alone (rows count baselines
+ * times timeslots, the window may cut a timeslot; robust_cost_func_batch,
+ * robust_batchmode_lbfgs.c:822-846).  A window with nrows <= 0 is empty: cost 0. */
+double dirac_b200_cost_window(dirac_b200_problem *pr, const double *pp, long long row0,
+                              long long nrows, double nu);
+/* gradient of that cost over the same rows, in the sign of the reference's minibatch gradient
+ * (robust_grad_func_batch, robust_batchmode_lbfgs.c:347-600): the NEGATIVE of what
+ * dirac_b200_grad(robust=1) returns for those rows; g has 8*N*Mt doubles, 0 for an empty window. */
+void dirac_b200_grad_window(dirac_b200_problem *pr, const double *pp, double *g, long long row0,
+                            long long nrows, double nu);
 /* per-cluster normal equations at pblk (8N doubles) for hybrid chunk `chunk` of cluster `clus`
  * against the hidden data xd (API layout, full interval): JTJ (8N x 8N), JTe (8N), returns
  * ||e||^2.  Equivalent of mylm_jac_single_pth + dgemm/dgemv (lmfit.c:484, clmfit.c:307-315). */

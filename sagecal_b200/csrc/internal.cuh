@@ -226,6 +226,10 @@ struct GradArgs {
   int robust;                // 0: R = e ; 1: R_i = e_i/(nu + e_i^2)
   double nu;
   double scale;              // +2 (Gaussian convention of robust_lbfgs.c:554) or -2 (robust, :299)
+  // row window of k_grad_tma_window: time blocks tb0, tb0+1, ... (gridDim.y of them), and only the
+  // rows [w_lo, w_hi) of the interval contribute (the full-interval kernel reads neither)
+  int tb0;
+  long long w_lo, w_hi;
 };
 
 struct ClusterPassArgs {
@@ -299,6 +303,8 @@ struct StreamAllArgs {
   int partial;
   long long row0;            // absolute row of the first row the pointers address (time-chunked
                              // launches shift the base pointers; hybrid chunk maps need the row)
+  long long w_lo, w_hi;      // MODE 2: rows [w_lo, w_hi) of the launch (relative to the shifted
+                             // pointers) are evaluated, the others of its timeslots are skipped
 };
 
 struct GramArgs {
@@ -357,6 +363,9 @@ void db_launch_coh_from_planar(const double2 *src, double2 *dst, long long r0, i
 void db_launch_vis_to_planar(const double2 *src, double2 *dst, long long R, cudaStream_t st);
 void db_launch_vis_from_planar(const double2 *src, double2 *dst, long long R, cudaStream_t st);
 void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st);
+// the gradient of rows [r_lo, r_hi) only: the time blocks that overlap them
+void db_launch_grad_window_tma(const GradArgs *a, int ntile, long long r_lo, long long r_hi,
+                               cudaStream_t st);
 int db_cluster_pass_nblocks(int ntile, int nt, int tslice);
 void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st);
 // whether plain (unweighted) passes of this array take k_cluster_pass_lin, the one variant that
@@ -384,6 +393,7 @@ void db_launch_bigtri_solve(const double *L, int ld, int n, const double *b, dou
                             unsigned epoch, int invert, cudaStream_t st);
 int db_stream_all_nblocks(int Nbase, int tilesz);
 void db_launch_predict_tma(const StreamAllArgs *a, cudaStream_t st);
+void db_launch_cost_window_tma(const StreamAllArgs *a, cudaStream_t st);
 void db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st);
 // (TB, NST, WARPS) of the last k_stream_all<1> launch since the reset (-1 each: none)
 void db_line_setup_shape_reset();

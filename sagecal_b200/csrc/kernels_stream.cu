@@ -150,10 +150,12 @@ __device__ __forceinline__ double warp_reduce4(double v0, double v1, double v2, 
 // warps per CTA share the 8 rings (the two warps of a station p consume the same stages; warp h=0
 // is the producer, the CTA barriers of the per-cluster reduction make a consumed stage reusable).
 // threadIdx.x = h*256 + w*32 + lane.
+// WIN: the gradient of the row window [a.w_lo, a.w_hi) alone (robust_grad_func_batch,
+// robust_batchmode_lbfgs.c:347-500): the grid's time blocks start at a.tb0, and rows outside the
+// window count like flagged rows (their residual is not read).
 // ------------------------------------------------------------------------------------------------
-template <int TB, int NST>
-__global__ void __launch_bounds__(2 * TILE_THREADS)
-k_grad_tma_split(GradArgs a) {
+template <int TB, int NST, bool WIN>
+__device__ __forceinline__ void grad_tma_split_body(GradArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int STAGE_ELEMS = TB * 4 * 32;  // double2 per stage
   double (*sq)[8][TILE_Q] = reinterpret_cast<double (*)[8][TILE_Q]>(smem_raw);
@@ -166,7 +168,7 @@ k_grad_tma_split(GradArgs a) {
   const int q0 = td.qb * TILE_Q;
   const int q = q0 + lane;
   const bool valid = (q > p) && (q < a.N);
-  const int t0 = blockIdx.y * TB;
+  const int t0 = (WIN ? a.tb0 + (int)blockIdx.y : (int)blockIdx.y) * TB;
   const int nrows = min(TB, a.tilesz - t0);
   const int qs = max(q0, p + 1);
   const int nv = max(0, min(q0 + TILE_Q, a.N) - qs);
@@ -206,6 +208,7 @@ k_grad_tma_split(GradArgs a) {
     const int t = t0 + i;
     const long long row = (long long)(t < a.tilesz ? t : a.tilesz - 1) * a.Nbase + b;
     use[i] = valid && (t < a.tilesz) && (a.flag[row] == 0);
+    if (WIN) use[i] = use[i] && row >= a.w_lo && row < a.w_hi;
 #pragma unroll
     for (int j = 0; j < 2; j++) {
       double2 e = make_double2(0.0, 0.0);
@@ -319,6 +322,18 @@ k_grad_tma_split(GradArgs a) {
       i0 = i1;
     }
   }
+}
+
+template <int TB, int NST>
+__global__ void __launch_bounds__(2 * TILE_THREADS)
+k_grad_tma_split(GradArgs a) {
+  grad_tma_split_body<TB, NST, false>(a);
+}
+
+template <int TB, int NST>
+__global__ void __launch_bounds__(2 * TILE_THREADS)
+k_grad_tma_window(GradArgs a) {
+  grad_tma_split_body<TB, NST, true>(a);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -885,6 +900,28 @@ void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st) {
   }
   dim3 grid(ntile, (a->tilesz + TB - 1) / TB);
   k_grad_tma_split<TB, NST><<<grid, 2 * TILE_THREADS, smem, st>>>(*a);
+}
+
+void db_launch_grad_window_tma(const GradArgs *a, int ntile, long long r_lo, long long r_hi,
+                               cudaStream_t st) {
+  constexpr int TB = 4, NST = 2;
+  if (r_hi <= r_lo) return;
+  const size_t smem = sizeof(double) * 2 * TILE_P * 8 * TILE_Q +
+                      (size_t)TILE_P * NST * TB * 4 * 32 * sizeof(double2) + TILE_P * NST * 8;
+  static bool configured = false;
+  if (!configured) {
+    DB_CHECK(cudaFuncSetAttribute(k_grad_tma_window<TB, NST>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured = true;
+  }
+  const int t_lo = (int)(r_lo / a->Nbase), t_hi = (int)((r_hi + a->Nbase - 1) / a->Nbase);
+  const int tb_lo = t_lo / TB, tb_hi = (t_hi + TB - 1) / TB;
+  GradArgs b = *a;
+  b.tb0 = tb_lo;
+  b.w_lo = r_lo;
+  b.w_hi = r_hi;
+  dim3 grid(ntile, tb_hi - tb_lo);
+  k_grad_tma_window<TB, NST><<<grid, 2 * TILE_THREADS, smem, st>>>(b);
 }
 
 // the linear-mapped kernel keeps 8N station sums in shared memory next to its ring and one arrival

@@ -3,6 +3,9 @@
 //   MODE 0  model over all clusters, residual / cost      (predict_threadfn_withgain_full,
 //           lmfit.c:611-688, plus cost_func / robust_cost_func, robust_lbfgs.c:674-726)
 //   MODE 1  line model V0,V1,V2 -> E0,E1,E2 of the LBFGS line search (kernels_line.cu)
+//   MODE 2  MODE 0 over a row window [w_lo, w_hi) of the launched timeslots: the cost and residual
+//           of the minibatch LBFGS (robust_cost_func_batch, robust_batchmode_lbfgs.c:822-846); rows
+//           of the first and last timeslot outside the window are neither written nor summed
 //
 // Why a ring: a pass that loads the coherencies into registers holds them there until they are
 // used, so registers bound it to few resident warps, and each warp waits out the full DRAM latency
@@ -29,7 +32,7 @@ k_stream_all(StreamAllArgs a) {
   // memory in warp order (deterministic), warp 0 finishes the rows.
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int STAGE_ELEMS = TB * 4 * 32;                       // double2 per stage
-  constexpr int NACC = (MODE == 0) ? 1 : 3;                       // V0 | V0,V1,V2
+  constexpr int NACC = (MODE == 1) ? 3 : 1;                       // V0 | V0,V1,V2
   constexpr size_t RING_BYTES = (size_t)WARPS * NST * STAGE_ELEMS * 16;
   constexpr size_t COMB_BYTES = (size_t)(WARPS - 1) * NACC * STAGE_ELEMS * 16;
   constexpr size_t DATA_BYTES = RING_BYTES > COMB_BYTES ? RING_BYTES : COMB_BYTES;
@@ -177,13 +180,14 @@ k_stream_all(StreamAllArgs a) {
     for (int i = 0; i < TB; i++) {
       if (i < nrows) {
         const long long row = (long long)(t0 + i) * a.Nbase + b;
+        if (MODE == 2 && (row < a.w_lo || row >= a.w_hi)) continue;
         const bool fl = a.flag[row] != 0;
 #pragma unroll
         for (int c = 0; c < 4; c++) {
           const long long ix = (long long)c * a.R + row;
           const double2 z = make_double2(0.0, 0.0);
           const double2 m = fl ? z : V0[i][c];
-          if (MODE == 0) {
+          if (MODE != 1) {
             double2 xv = z;
             if (a.out_mode == 1 || a.cost_mode) xv = ld_stream(a.x + ix);
             const double2 e = csub(xv, m);
@@ -206,7 +210,7 @@ k_stream_all(StreamAllArgs a) {
       }
     }
   }
-  if (MODE == 0 && a.cost_mode) {
+  if (MODE != 1 && a.cost_mode) {
     // deterministic grid reduction (per-CTA partial from warp 0, last CTA sums in index order)
     __shared__ bool is_last;
     cost = warp_sum(cost);
@@ -240,7 +244,7 @@ static void launch_cfg(const StreamAllArgs *a, cudaStream_t st) {
   }
   const int nbg = (a->Nbase + 31) / 32, ntb = (a->tilesz + TB - 1) / TB;
   const unsigned grid = (unsigned)((long long)nbg * ntb);
-  constexpr int NACC = (MODE == 0) ? 1 : 3;
+  constexpr int NACC = (MODE == 1) ? 3 : 1;
   const size_t ring = (size_t)WARPS * NST * TB * 4 * 32 * 16;
   const size_t comb = (size_t)(WARPS - 1) * NACC * TB * 4 * 32 * 16;
   const size_t smem = (ring > comb ? ring : comb) + WARPS * NST * 8;
@@ -261,6 +265,11 @@ int db_stream_all_nblocks(int Nbase, int tilesz) {
 }
 void db_launch_predict_tma(const StreamAllArgs *a, cudaStream_t st) {
   launch_cfg<0, 2, 2, 3>(a, st);
+}
+// the caller shifts the pointers to the first timeslot of the window and sets tilesz to the
+// timeslots it touches; the grid, and the cost's grid reduction, cover those timeslots only
+void db_launch_cost_window_tma(const StreamAllArgs *a, cudaStream_t st) {
+  launch_cfg<2, 2, 2, 3>(a, st);
 }
 void db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st) {
   // one row per item keeps the three accumulated polynomials of the line model at 24 registers

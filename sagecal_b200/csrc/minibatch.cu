@@ -107,6 +107,41 @@ struct MultiChan {
   }
 };
 
+// ---- the stochastic closing stage of sagefit (lbfgs_m < 0, robust modes) ------------------------------
+// Cost and gradient of one row window of the resident interval: the windowed passes of problem.cu
+// stream only the timeslots the window overlaps.  The iterate and the two-loop recursion stay on the
+// host, as in bfgsfit_minibatch_visibilities.
+struct RowWindow {
+  dirac_b200_problem *pr;
+  double nu;
+  long long r0, nr;
+  void set_window(long long row0, long long nrows) {
+    r0 = row0;
+    nr = nrows;
+  }
+  double cost(const double *p) {
+    if (nr <= 0) return 0.0;
+    return dirac_b200_cost_window(pr, p, r0, nr, nu);
+  }
+  void grad(const double *p, double *g) {
+    if (nr <= 0) {
+      memset(g, 0, sizeof(double) * pr->d.npar);
+      return;
+    }
+    dirac_b200_grad_window(pr, p, g, r0, nr, nu);
+  }
+};
+
+// lbfgs_fit_robust_wrapper_minibatch on the resident problem (lmfit.c:1027-1029); p: host, npar, in/out
+void db_lbfgs_fit_minibatch(dirac_b200_problem *pr, double *p, int m, int itmax, int M, double nu) {
+  RowWindow F;
+  F.pr = pr;
+  F.nu = nu;
+  F.r0 = 0;
+  F.nr = pr->d.R;
+  minibatch::lbfgs_fit_robust_wrapper_minibatch(F, p, m, pr->d.R, itmax, M);
+}
+
 static int minibatch_fit(double *x, int N, int Nbase, int tilesz, baseline_t *barr,
                          clus_source_t *carr, double *coh, int M, int Mt, int Nf, double *p,
                          const double *y, const double *z, const double *rho, int max_lbfgs,

@@ -1,7 +1,9 @@
 // Minibatch (stochastic) LBFGS of the reference, restated decision for decision, templated on the
 // function object that supplies cost and gradient (lbfgs_fit_minibatch, linesearch_backtrack,
 // mult_hessian: lbfgs.c:717-930, 444-474, 33-111).  The product instantiates it with the multi-channel
-// device evaluator (minibatch.cu); oracle/minibatch_harness.cpp instantiates it with the oracle's
+// device evaluator and, through lbfgs_fit_robust_wrapper_minibatch, with the row windows of a resident
+// interval (sagefit's stochastic stage, minibatch.cu; pinned on the CPU by
+// tests/test_oracle_minibatch_window.py); oracle/minibatch_harness.cpp instantiates it with the oracle's
 // per-row cost / gradient to pin the control flow against the compiled reference without a GPU (test
 // infrastructure, not shipped).
 //
@@ -154,6 +156,41 @@ void lbfgs_fit_minibatch(FN &F, double *p, int m, int itmax, int M,
     }
   }
   memcpy(p, xk.data(), sizeof(double) * m);
+}
+
+// Batch table of the stochastic stage of sagefit (lbfgs_persist_init, lbfgs.c:954-1010, with the
+// n rows of the interval): window i is the rows [i b, i b + len_i), b = ceil(n / nbatch),
+// len_i = min(b, n - i b).  len_i <= 0 (fewer rows than windows) is an empty window.
+inline void batch_window(long long n, int nbatch, int i, long long *off, long long *len) {
+  const long long b = (n + nbatch - 1) / nbatch;
+  *off = (long long)i * b;
+  *len = (n - *off < b) ? n - *off : b;
+}
+
+// lbfgs_fit_robust_wrapper_minibatch (robust_batchmode_lbfgs.c:859-930): (itmax + 4) / 4 epochs over
+// the 5 row windows of the interval in order, 4 minibatch iterations per window, one persistent state
+// (curvature pairs, gradient running averages) created for this call and carried through all of them.
+// FW: the F concept plus  void set_window(long long row0, long long nrows);
+template <class FW>
+void lbfgs_fit_robust_wrapper_minibatch(FW &F, double *p, int m, long long nrows, int itmax,
+                                        int M) {
+  const int Nbatch = 5, Niterperbatch = 4;
+  std::vector<double> s((size_t)m * (M + 2) + 8, 0.0), y((size_t)m * M + 1, 0.0), rho(M + 1, 0.0);
+  persistent_data_t pt;
+  memset(&pt, 0, sizeof(pt));
+  pt.s = s.data();
+  pt.y = y.data();
+  pt.rho = rho.data();
+  pt.m = m;
+  pt.lbfgs_m = M;
+  const int Nloops = (itmax + Niterperbatch) / Niterperbatch;
+  for (int nl = 0; nl < Nloops; nl++)
+    for (int ci = 0; ci < Nbatch; ci++) {
+      long long off, len;
+      batch_window(nrows, Nbatch, ci, &off, &len);
+      F.set_window(off, len);
+      lbfgs_fit_minibatch(F, p, m, Niterperbatch, M, &pt);
+    }
 }
 
 

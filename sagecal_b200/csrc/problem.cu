@@ -499,6 +499,82 @@ void db_grad_dev(dirac_b200_problem *pr, const double *pp_dev, double *g_dev, in
   db_allreduce(pr, g_dev, d.npar);
 }
 
+// Student's-t cost of the rows [r_lo, r_hi) alone at pp_dev (robust_cost_func_batch,
+// robust_batchmode_lbfgs.c:822-846): only the timeslots that overlap the window are streamed, rows of
+// the first and last of them outside it are skipped.  out != null: the residual e = x - V of the
+// window's rows is written there (the other rows of out are left as they are).  Returns the cost.
+double db_cost_window_dev(dirac_b200_problem *pr, const double *pp_dev, double2 *out, double nu,
+                          long long r_lo, long long r_hi) {
+  DevProblem &d = pr->d;
+  if (r_lo < 0) r_lo = 0;
+  if (r_hi > d.R) r_hi = d.R;
+  if (r_hi <= r_lo) return 0.0;  // an empty window of the batch table
+  const long long t_lo = r_lo / d.Nbase, t_hi = (r_hi + d.Nbase - 1) / d.Nbase;
+  const long long r0 = t_lo * d.Nbase, len = r_hi - r_lo;
+  StreamAllArgs a;
+  memset(&a, 0, sizeof(a));
+  a.coh = d.coh + r0; a.x = d.x + r0; a.flag = d.flag + r0; a.pp = pp_dev; a.clus = d.clus;
+  a.chunk_poff = d.chunk_poff; a.blpq = d.blpq; a.partials = pr->partials;
+  a.cost = d.scal; a.counter = d.counters; a.R = d.R; a.N = d.N; a.Nbase = d.Nbase;
+  a.tilesz = (int)(t_hi - t_lo); a.M = d.M; a.row0 = r0;
+  a.w_lo = r_lo - r0; a.w_hi = r_hi - r0;
+  a.inv_nu = (nu > 0.0) ? 1.0 / nu : 0.0;
+  const double bytes = (double)len * (64.0 * d.M + 65.0 + (out ? 64.0 : 0.0));
+  if (pr->world <= 1) {
+    a.out = out ? out + r0 : nullptr;
+    a.out_mode = out ? 1 : 0;
+    a.cost_mode = 2;
+    db_prof_begin(0, bytes, d.stream);
+    db_launch_cost_window_tma(&a, d.stream);
+    db_prof_end(d.stream);
+    db_count_launch(1);
+    return db_read_scalar(pr, 0);
+  }
+  // cluster-sharded: partial model of the local clusters over the window, its 8 len doubles summed
+  // over the ranks, then residual and cost of each polarisation plane from the sum (identical on
+  // every rank; the four plane costs are added on the host in plane order)
+  if (!pr->pm) pr->pm = dev_alloc<double2>((size_t)4 * d.R);
+  a.out = pr->pm + r0; a.out_mode = 2; a.cost_mode = 0;
+  db_prof_begin(0, bytes, d.stream);
+  db_launch_cost_window_tma(&a, d.stream);
+  db_prof_end(d.stream);
+  for (int c = 0; c < 4; c++) db_allreduce(pr, pr->pm + (long long)c * d.R + r_lo, 2 * len);
+  for (int c = 0; c < 4; c++) {
+    const long long off = (long long)c * d.R + r_lo;
+    db_launch_residual_cost(d.x + off, pr->pm + off, out ? out + off : nullptr, len, out ? 1 : 0, 2,
+                            a.inv_nu, pr->partials, d.scal + 32 + c, d.counters, d.stream);
+  }
+  db_count_launch(5);
+  DB_CHECK(cudaMemcpyAsync(d.h_scal + 32, d.scal + 32, 4 * sizeof(double), cudaMemcpyDeviceToHost,
+                           d.stream));
+  db_stream_sync(d.stream);
+  return ((d.h_scal[32] + d.h_scal[33]) + d.h_scal[34]) + d.h_scal[35];
+}
+
+// gradient of the Student's-t cost over the rows [r_lo, r_hi) alone, from the residual of those rows
+// in pr->res, with the sign of the reference's minibatch gradient (func_grad_robust_batch,
+// robust_batchmode_lbfgs.c:489: -2 sum xr dV/(nu + xr^2) with xr = model - data, the NEGATED true
+// gradient); g_dev (npar) is overwritten
+void db_grad_window_dev(dirac_b200_problem *pr, const double *pp_dev, double *g_dev, double nu,
+                        long long r_lo, long long r_hi) {
+  DevProblem &d = pr->d;
+  if (r_lo < 0) r_lo = 0;
+  if (r_hi > d.R) r_hi = d.R;
+  DB_CHECK(cudaMemsetAsync(g_dev, 0, sizeof(double) * d.npar, d.stream));
+  if (r_hi <= r_lo) return;  // (the same window on every rank)
+  GradArgs a;
+  memset(&a, 0, sizeof(a));
+  a.coh = d.coh; a.res = pr->res; a.flag = d.flag; a.pp = pp_dev; a.clus = d.clus;
+  a.chunk_poff = d.chunk_poff; a.tiles = d.tiles; a.g = g_dev; a.R = d.R; a.N = d.N;
+  a.Nbase = d.Nbase; a.tilesz = d.tilesz; a.M = d.M; a.robust = 1; a.nu = nu;
+  a.scale = 2.0;  // e = d - f:  -2 (f - d) = +2 e
+  db_prof_begin(1, (double)(r_hi - r_lo) * (64.0 * d.M + 65.0) + 64.0 * d.N * d.Mt, d.stream);
+  db_launch_grad_window_tma(&a, d.ntile, r_lo, r_hi, d.stream);
+  db_prof_end(d.stream);
+  db_count_launch(1);
+  db_allreduce(pr, g_dev, d.npar);
+}
+
 // ------------------------------------------------------------------------------------------------
 // thin C-ABI
 // ------------------------------------------------------------------------------------------------
@@ -526,6 +602,27 @@ extern "C" void dirac_b200_grad(dirac_b200_problem *pr, const double *pp, double
   db_grad_dev(pr, d.pp, pr->g, robust, nu);
   DB_CHECK(cudaMemcpyAsync(g, pr->g, sizeof(double) * d.npar, cudaMemcpyDeviceToHost,
                            d.stream));
+  db_stream_sync(d.stream);
+  DB_CHECK(cudaGetLastError());
+}
+
+extern "C" double dirac_b200_cost_window(dirac_b200_problem *pr, const double *pp, long long row0,
+                                         long long nrows, double nu) {
+  DevProblem &d = pr->d;
+  DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * d.npar, cudaMemcpyHostToDevice, d.stream));
+  const double c = db_cost_window_dev(pr, d.pp, nullptr, nu, row0, row0 + nrows);
+  db_stream_sync(d.stream);
+  DB_CHECK(cudaGetLastError());
+  return c;
+}
+
+extern "C" void dirac_b200_grad_window(dirac_b200_problem *pr, const double *pp, double *g,
+                                       long long row0, long long nrows, double nu) {
+  DevProblem &d = pr->d;
+  DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * d.npar, cudaMemcpyHostToDevice, d.stream));
+  db_cost_window_dev(pr, d.pp, pr->res, nu, row0, row0 + nrows);  // residual of the window's rows
+  db_grad_window_dev(pr, d.pp, pr->g, nu, row0, row0 + nrows);
+  DB_CHECK(cudaMemcpyAsync(g, pr->g, sizeof(double) * d.npar, cudaMemcpyDeviceToHost, d.stream));
   db_stream_sync(d.stream);
   DB_CHECK(cudaGetLastError());
 }

@@ -100,6 +100,11 @@ void db_predict_dev(dirac_b200_problem *pr, const double *pp_dev, double2 *out, 
 double db_read_scalar(dirac_b200_problem *pr, int slot);
 void db_grad_dev(dirac_b200_problem *pr, const double *pp_dev, double *g_dev, int robust,
                  double nu);
+// Student's-t cost and minibatch-sign gradient of the row window [r_lo, r_hi) (problem.cu)
+double db_cost_window_dev(dirac_b200_problem *pr, const double *pp_dev, double2 *out, double nu,
+                          long long r_lo, long long r_hi);
+void db_grad_window_dev(dirac_b200_problem *pr, const double *pp_dev, double *g_dev, double nu,
+                        long long r_lo, long long r_hi);
 void db_lm_init(dirac_b200_problem *pr);
 void db_prefactor_sweep(dirac_b200_problem *pr, double tau);
 void db_allreduce(dirac_b200_problem *pr, void *dev, long long count);

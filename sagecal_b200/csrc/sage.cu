@@ -22,6 +22,7 @@ bool db_cluster_needs_rowmap(const dirac_b200_problem *pr, int k);
 void db_cluster_hidden(dirac_b200_problem *pr, int k, double2 *r, int sign);
 void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
                   double nu);
+void db_lbfgs_fit_minibatch(dirac_b200_problem *pr, double *p, int m, int itmax, int M, double nu);
 void db_rtr_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, double2 *r, int kind,
                   int itmax_a, int itmax_b, double nulow, double nuhigh, double *robust_nu,
                   double *info, bool hidden_ready, const double *aug_y, const double *aug_bz,
@@ -249,9 +250,8 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
       if (lbfgs_m > 0) {
         db_lbfgs_fit(pr, pp, m, max_lbfgs, lbfgs_m, 1, robust_nu0);
       } else if (lbfgs_m < 0) {
-        fprintf(stderr, "dirac_b200: minibatch LBFGS (lbfgs_m<0) is not supported; running "
-                        "full-batch with memory %d\n", -lbfgs_m);
-        db_lbfgs_fit(pr, pp, m, max_lbfgs, -lbfgs_m, 1, robust_nu0);
+        // stochastic LBFGS over 5 row windows of the interval (lmfit.c:1027-1029)
+        db_lbfgs_fit_minibatch(pr, pp, m, max_lbfgs, -lbfgs_m, robust_nu0);
       }
     } else {
       db_lbfgs_fit(pr, pp, m, max_lbfgs, lbfgs_m, 0, 0.0);

@@ -19,7 +19,8 @@ EXPORTED = [
     "precalculate_coherencies", "predict_visibilities_multifreq", "generate_baselines",
     "preset_flags_and_data", "whiten_data", "dirac_b200_create", "dirac_b200_destroy", "dirac_b200_set_data",
     "dirac_b200_precalculate", "dirac_b200_get_coherencies", "dirac_b200_predict",
-    "dirac_b200_grad", "dirac_b200_normal_eq", "dirac_b200_launch_count", "dirac_b200_sagefit",
+    "dirac_b200_grad", "dirac_b200_cost_window", "dirac_b200_grad_window", "dirac_b200_normal_eq",
+    "dirac_b200_launch_count", "dirac_b200_sagefit",
     "dirac_b200_set_stream", "dirac_b200_profile_enable", "dirac_b200_profile_read",
     "dirac_b200_kernel_count", "dirac_b200_normal_eq_weighted", "dirac_b200_create_shard",
     "dirac_b200_set_comm", "dirac_b200_spd_solve", "dirac_b200_tri_solve", "dirac_b200_tri_solve_ld",
@@ -66,6 +67,9 @@ class DiracB200(DiracAPI):
         L.dirac_b200_predict.restype = d
         L.dirac_b200_predict.argtypes = [vp, dp, dp, i, i, d]
         L.dirac_b200_grad.argtypes = [vp, dp, dp, i, d]
+        L.dirac_b200_cost_window.restype = d
+        L.dirac_b200_cost_window.argtypes = [vp, dp, C.c_longlong, C.c_longlong, d]
+        L.dirac_b200_grad_window.argtypes = [vp, dp, dp, C.c_longlong, C.c_longlong, d]
         L.dirac_b200_normal_eq.restype = d
         L.dirac_b200_normal_eq.argtypes = [vp, i, i, dp, dp, dp, dp]
         L.dirac_b200_normal_eq_weighted.restype = d
@@ -213,6 +217,16 @@ class DeviceProblem:
     def grad(self, pp, robust=False, nu=0.0):
         g = np.zeros(self.m)
         self.api.lib.dirac_b200_grad(self.h, dptr(pp), dptr(g), 1 if robust else 0, nu)
+        return g
+
+    def cost_window(self, pp, row0, nrows, nu):
+        """Student's-t cost of the rows [row0, row0 + nrows) alone"""
+        return self.api.lib.dirac_b200_cost_window(self.h, dptr(pp), row0, nrows, nu)
+
+    def grad_window(self, pp, row0, nrows, nu):
+        """gradient of cost_window with the reference's minibatch sign (minus the true gradient)"""
+        g = np.zeros(self.m)
+        self.api.lib.dirac_b200_grad_window(self.h, dptr(pp), dptr(g), row0, nrows, nu)
         return g
 
     def sagefit(self, pp, x_out=None, max_emiter=3, max_iter=2, max_lbfgs=10, lbfgs_m=7, linsolv=0,
