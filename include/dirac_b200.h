@@ -524,4 +524,7 @@ int dirac_b200_bigtri_solve(int n, const double *L, const double *b, double *x, 
 #ifdef __cplusplus
 }
 #endif
+
+/* simulation with solutions (predict_visibilities_multifreq_withsol and its beam variants) */
+#include "dirac_b200_withsol.h"
 #endif

@@ -42,13 +42,13 @@ struct CohArgs {
   double2 *coh;              // MODE 0 out: planar [M][4][R]
   unsigned char *flag;       // MODE 0: uv-cut flags (may be null)
   double2 *xout;             // MODE 1, 2 in/out: [Nchan][R][4]
-  // MODE 2 (full-resolution residual with solutions, residual.c:681-938)
+  // MODE 2 (full-resolution residual / simulation with solutions, residual.c:681-938,1342-1618)
   const int *sta1, *sta2;        // [R] stations of every row
   const double *p;               // Jones solutions (layout of pp)
   const int *clus_nchunk;        // [M]
   const int *clus_chunk0;        // [M] first entry of cluster k in chunk_poff
   const int *chunk_poff;         // [Mt]
-  const unsigned char *clus_sub; // [M] 1: subtract this cluster (id >= 0)
+  const signed char *clus_coef;  // [M] sign of J C J^H in x: -1 subtract, +1 add, 0 skip the cluster
   const double *pinv;            // inverse Jones of the correction cluster [nchunk][N][8], or null
   int pinv_nchunk, N;
   // station beams (predict_withbeam.c:300-420): tables per (timeslot, channel, source, station) made

@@ -18,9 +18,11 @@
 #define COH_THREADS 128
 
 // MODE 0: coherencies per cluster at freq[0] -> planar coh ; MODE 1: multifreq sum -> xout ;
-// MODE 2: xout -= sum_k J_p C_k J_q^H per channel with the solved Jones (clusters with id >= 0), then
-//         the optional correction x <- Jinv_p x Jinv_q^H by one cluster's inverse Jones
-//         (residual_threadfn_multifreq, residual.c:681-938)
+// MODE 2: xout += sum_k clus_coef[k] J_p C_k J_q^H per channel with the solved Jones, then the
+//         optional correction x <- Jinv_p x Jinv_q^H by one cluster's inverse Jones.  The residual
+//         passes -1 for clusters with id >= 0 (residual_threadfn_multifreq, residual.c:681-938), the
+//         simulation +1 / -1 for the clusters not ignored (predictwithgain_threadfn_multifreq,
+//         residual.c:1344-1618); 0 skips a cluster.
 template <int MODE>
 __global__ void __launch_bounds__(COH_THREADS)
 k_sky_predict(CohArgs a) {
@@ -129,7 +131,7 @@ k_sky_predict(CohArgs a) {
           } else if (MODE == 1) {
 #pragma unroll
             for (int c = 0; c < 4; c++) X[c] = cadd(X[c], C[c]);
-          } else if (a.clus_sub[sg.cluster]) {
+          } else if (const int coef = a.clus_coef[sg.cluster]) {
             // Jones of this row's hybrid chunk: px = row / ceil(R / nchunk)  (residual.c:717)
             const int nch = a.clus_nchunk[sg.cluster];
             const int px = row_chunk(r, a.R, nch);
@@ -139,8 +141,9 @@ k_sky_predict(CohArgs a) {
             load_jones(pm, s2, G2);
             mat_ab(G1, C, T1);
             mat_abh(T1, G2, T2);
+            // (X - T and X + (-T) round alike: a negative coefficient subtracts bit for bit)
 #pragma unroll
-            for (int c = 0; c < 4; c++) X[c] = csub(X[c], T2[c]);
+            for (int c = 0; c < 4; c++) X[c] = coef < 0 ? csub(X[c], T2[c]) : cadd(X[c], T2[c]);
           }
 #pragma unroll
           for (int c = 0; c < 4; c++) C[c] = make_double2(0.0, 0.0);

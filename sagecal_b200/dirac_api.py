@@ -218,6 +218,13 @@ def make_barr(sta1, sta2, flag):
     return barr
 
 
+def _ignorelist(ignorelist, M):
+    """the int[M] ignore list of the simulation calls; None: no cluster ignored"""
+    ign = np.zeros(M, dtype=np.int32) if ignorelist is None else np.asarray(ignorelist, dtype=np.int32)
+    assert ign.shape == (M,)
+    return np.ascontiguousarray(ign)
+
+
 def barr_to_numpy(barr, n):
     view = np.ctypeslib.as_array(C.cast(barr, C.POINTER(C.c_int)), shape=(n, 3))
     fl = np.ctypeslib.as_array(C.cast(barr, c_ubyte_p), shape=(n, 12))
@@ -251,6 +258,9 @@ class DiracAPI:
         L.calculate_residuals_multifreq.restype = i
         L.calculate_residuals_multifreq.argtypes = [dp, dp, dp, dp, dp, i, i, i, bp, cp, i, dp, i,
                                                     d, d, d, i, i, d, i]
+        L.predict_visibilities_multifreq_withsol.restype = i
+        L.predict_visibilities_multifreq_withsol.argtypes = [dp, dp, dp, dp, dp, c_int_p, i, i, i, bp,
+                                                             cp, i, dp, i, d, d, d, i, i, i, d, i]
         L.generate_baselines.restype = i
         L.generate_baselines.argtypes = [i, i, i, bp, i]
         L.preset_flags_and_data.restype = i
@@ -300,6 +310,20 @@ class DiracAPI:
             dptr(u), dptr(v), dptr(w), dptr(p), dptr(x), N, Nbase, tilesz, barr, sky.arr, sky.M,
             dptr(freqs), len(freqs), fdelta, tdelta, dec0, Nt, ccid, rho, phase_only)
 
+    def predict_visibilities_multifreq_withsol(self, u, v, w, p, x, N, Nbase, tilesz, barr,
+                                               sky: SkyModel, freqs, fdelta, ignorelist=None,
+                                               tdelta=10.0, dec0=1.0, Nt=4, add_to_data=1,
+                                               ccid=-99999, rho=1e-9, phase_only=0):
+        """simulation with solutions (Dirac_radio.h:666).  x[chan][row][8] in/out; ignorelist: one
+        flag per cluster position, nonzero skips the cluster (None: predict every cluster);
+        add_to_data 1 model only, 2 add, 3 subtract; then the optional correction by cluster ccid"""
+        freqs = np.ascontiguousarray(freqs, dtype=np.float64)
+        ign = _ignorelist(ignorelist, sky.M)
+        return self.lib.predict_visibilities_multifreq_withsol(
+            dptr(u), dptr(v), dptr(w), dptr(p), dptr(x), ign.ctypes.data_as(c_int_p), N, Nbase,
+            tilesz, barr, sky.arr, sky.M, dptr(freqs), len(freqs), fdelta, tdelta, dec0, Nt,
+            add_to_data, ccid, rho, phase_only)
+
     # ---- station beams (Dirac_radio.h:472-490) ----
     def precalculate_coherencies_withbeam(self, u, v, w, N, Nbase1, barr, sky, freq0, fdelta, beam,
                                           tdelta=10.0, dec0=1.0, uvmin=0.0, uvmax=1e9, Nt=4):
@@ -343,6 +367,22 @@ class DiracAPI:
             dptr(u), dptr(v), dptr(w), dptr(p), dptr(x), N, Nbase, tilesz, barr, sky.arr, sky.M,
             dptr(freqs), len(freqs), C.c_double(fdelta), C.c_double(tdelta), C.c_double(dec0),
             *beam.head(), *beam.tail(), Nt, ccid, C.c_double(rho), phase_only)
+
+    def predict_visibilities_multifreq_withsol_withbeam(self, u, v, w, p, x, N, Nbase, tilesz, barr,
+                                                        sky, freqs, fdelta, beam, ignorelist=None,
+                                                        tdelta=10.0, dec0=1.0, Nt=4, add_to_data=1,
+                                                        ccid=-99999, rho=1e-9, phase_only=0,
+                                                        gpu_twin=False):
+        """predict_visibilities_multifreq_withsol with station beams (Dirac_radio.h:490);
+        gpu_twin: through its GPU-build name predict_visibilities_withsol_withbeam_gpu (:529)"""
+        freqs = np.ascontiguousarray(freqs, dtype=np.float64)
+        ign = _ignorelist(ignorelist, sky.M)
+        fn = (self.lib.predict_visibilities_withsol_withbeam_gpu if gpu_twin
+              else self.lib.predict_visibilities_multifreq_withsol_withbeam)
+        return fn(dptr(u), dptr(v), dptr(w), dptr(p), dptr(x), ign.ctypes.data_as(c_int_p), N, Nbase,
+                  tilesz, barr, sky.arr, sky.M, dptr(freqs), len(freqs), C.c_double(fdelta),
+                  C.c_double(tdelta), C.c_double(dec0), *beam.head(), *beam.tail(), Nt, add_to_data,
+                  ccid, C.c_double(rho), phase_only)
 
     def sagefit_visibilities(self, u, v, w, x, N, Nbase, tilesz, barr, sky: SkyModel, coh, pp,
                              freq0=150e6, fdelta=195.3e3, uvmin=0.0, Nt=4, max_emiter=3,

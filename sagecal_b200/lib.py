@@ -40,6 +40,12 @@ EXPORTED = [
     "bfgsfit_minibatch_visibilities_hbb", "bfgsfit_minibatch_consensus_hbb", "dirac_b200_barr_from_hbb",
 ]
 
+#: every symbol include/dirac_b200_withsol.h declares (simulation with solutions)
+WITHSOL_EXPORTED = [
+    "predict_visibilities_multifreq_withsol", "predict_visibilities_multifreq_withsol_withbeam",
+    "predict_visibilities_withsol_withbeam_gpu",
+]
+
 
 class DiracB200(DiracAPI):
     """The product library: the reference entry points (inherited bindings) plus the thin
