@@ -170,9 +170,11 @@ k_sky_predict(CohArgs a) {
     }
   }
   if (MODE == 0 && active && a.flag) {
-    // uv cut: unflagged rows outside [uvmin, uvmax] get flag 2 (predict.c:488-493)
+    // uv cut: unflagged rows outside [uvmin, uvmax] get flag 2 (predict.c:488-493).  u u and v v
+    // are rounded before they are added, as on the host: a fused multiply-add would move a row that
+    // lies on uvmin or uvmax by an ulp to the other side of the limit.
     if (a.flag[r] == 0) {
-      const double uvdist = sqrt(u * u + v * v) * a.freqs[0];
+      const double uvdist = sqrt(__dadd_rn(__dmul_rn(u, u), __dmul_rn(v, v))) * a.freqs[0];
       if (uvdist < a.uvmin || uvdist > a.uvmax) a.flag[r] = 2;
     }
   }

@@ -256,6 +256,218 @@ def split_cluster(cl, parts):
     return out
 
 
+#: element-wise error budget of the sky prediction: |got - want| <= SKY_C eps sum_s w_s per row,
+#: correlation and channel, w_s from sky_predict_ref
+SKY_C = 16.0
+
+
+def sky_predict_ref(u, v, w, clusters, freq, fdelta2, spectral):
+    """per-cluster coherencies of point, Gaussian, disk and ring sources at one frequency, restated in
+    long double from predict.c:399-472 (spectral=False: the fluxes sI..sV as they are) and
+    residual.c:1124-1226 (spectral=True: the three-term log spectral index from sI0..sV0 and f0 where
+    spec_idx != 0).  M_PI is the double constant, as in both codes.  returns (C [nrow, M, 4] complex,
+    budget [nrow, M]): budget is the sum over the cluster's sources of
+      w_s = |flux_s| (|shape_s| (1 + phi_s) + 1 + sigma_s + lambda_s),
+    |flux_s| = |I| + |Q| + |U| + |V|, phi_s = 2 pi f (|u l| + |v m| + |w n|) the size of the phase
+    before cancellation (G is rounded before it is scaled by f, so a phase of 1e5 rad carries an error
+    of about 1e5 eps), sigma_s the sensitivity of the shape factor to a relative error of its argument
+    (Gaussian x e^-x with x = 2 pi^2 (ut^2 + vt^2) taken over absolute values, disk / ring the Bessel
+    argument, |j0'|, |j1'| <= 1) and lambda_s = |log |s0|| + |tempfr| that of the spectral flux."""
+    from scipy import special
+    L = np.longdouble
+    pi = L(np.pi)
+    f = L(freq)
+    u = np.asarray(u, dtype=L)[:, None]
+    v = np.asarray(v, dtype=L)[:, None]
+    w = np.asarray(w, dtype=L)[:, None]
+    nrow = u.shape[0]
+    C = np.zeros((nrow, len(clusters), 4), dtype=np.clongdouble)
+    budget = np.zeros((nrow, len(clusters)))
+    for k, cl in enumerate(clusters):
+        K = len(cl["ll"])
+        if K == 0:
+            continue
+        ll, mm, nn = (np.asarray(cl[n], dtype=L)[None, :] for n in ("ll", "mm", "nn"))
+        G = 2 * pi * (u * ll + v * mm + w * nn)
+        phi = 2 * pi * f * (np.abs(u * ll) + np.abs(v * mm) + np.abs(w * nn))
+        ph = np.exp(1j * (G * f))
+        with np.errstate(invalid="ignore", divide="ignore"):
+            sm = G * L(fdelta2)
+            fac = np.where(G != 0, np.abs(np.sin(sm) / np.where(G != 0, sm, 1)), L(1))
+        ph = ph * fac
+        st = np.asarray(cl.get("stype", np.zeros(K)), dtype=int)
+        shape = np.ones((nrow, K), dtype=L)
+        sigma = np.zeros((nrow, K), dtype=L)
+        uf, vf, wf = u * f, v * f, w * f
+        gauss, disk = cl.get("gauss"), cl.get("disk") or {}
+        for s in range(K):
+            if st[s] == 0:
+                continue
+            if st[s] == 1:
+                eX, eY, eP, cxi, sxi, cphi, sphi, proj = (L(x) for x in gauss[s])
+            else:
+                eX, cxi, sxi, cphi, sphi, proj = (L(x) for x in disk[s])
+                proj = L(1)   # disks and rings always project (predict.c:67-68,82-83)
+            if proj != 0:
+                terms_u = (uf * cxi, -vf * cphi * sxi, wf * sphi * sxi)
+                terms_v = (uf * sxi, vf * cphi * cxi, -wf * sphi * cxi)
+            else:
+                terms_u, terms_v = (uf,), (vf,)
+            up, vp = sum(terms_u)[:, 0], sum(terms_v)[:, 0]
+            uvabs = (sum(np.abs(t) for t in terms_u) + sum(np.abs(t) for t in terms_v))[:, 0]
+            if st[s] == 1:
+                sP, cP = np.sin(L(float(eP))), np.cos(L(float(eP)))
+                ut = eX * (cP * up - sP * vp)
+                vt = eY * (sP * up + cP * vp)
+                x = 2 * pi * pi * (ut * ut + vt * vt)
+                shape[:, s] = np.exp(-x)
+                sigma[:, s] = 2 * pi * pi * (eX * eX + eY * eY) * uvabs * uvabs * np.exp(-x)
+            else:
+                b = np.sqrt(up * up + vp * vp) * eX * 2 * pi
+                bd = b.astype(np.float64)   # scipy's Bessel functions on the long-double argument
+                shape[:, s] = (special.j1 if st[s] == 2 else special.j0)(bd)
+                sigma[:, s] = 2 * pi * eX * uvabs + 1
+        ph = ph * shape
+        flux = [np.asarray(cl[n], dtype=L) for n in ("sI", "sQ", "sU", "sV")]
+        lam = np.zeros(K, dtype=L)
+        if spectral:
+            si = [np.asarray(cl.get(n, np.zeros(K)), dtype=L) for n in ("spec_idx", "spec_idx1",
+                                                                         "spec_idx2")]
+            f0 = np.asarray(cl.get("f0", np.full(K, 150e6)), dtype=L)
+            fr = np.log(f / f0)
+            tf = si[0] * fr + si[1] * fr * fr + si[2] * fr * fr * fr
+            tfa = np.abs(si[0] * fr) + np.abs(si[1] * fr * fr) + np.abs(si[2] * fr * fr * fr)
+            on = si[0] != 0
+            for j, n in enumerate(("sI0", "sQ0", "sU0", "sV0")):
+                s0 = np.asarray(cl.get(n, cl[n[:2]]), dtype=L)
+                with np.errstate(divide="ignore"):
+                    sf = np.where(s0 > 0, np.exp(np.log(np.abs(s0)) + tf),
+                                  np.where(s0 == 0, L(0), -np.exp(np.log(np.abs(s0)) + tf)))
+                    lj = np.where(s0 != 0, np.abs(np.log(np.abs(s0))), L(0))
+                flux[j] = np.where(on, sf, flux[j])
+                lam = np.maximum(lam, np.where(on, lj + tfa, L(0)))
+        I, Q, U, V = flux
+        C[:, k, 0] = ph @ (I + Q)
+        C[:, k, 1] = ph @ (U + 1j * V)
+        C[:, k, 2] = ph @ (U - 1j * V)
+        C[:, k, 3] = ph @ (I - Q)
+        fa = (np.abs(I) + np.abs(Q) + np.abs(U) + np.abs(V))[None, :]
+        ws = fa * (np.abs(shape) * (1 + phi) + 1 + sigma + lam[None, :])
+        budget[:, k] = np.sum(ws, axis=1).astype(np.float64)
+    return C, budget
+
+
+def sky_edge_case(name, seed=5):
+    """(u, v, w, clusters, freqs, fdelta) of one edge of the sky prediction, on the rows of
+    small_problem(N=6, tilesz=4) (60 rows), every source type of the restatement present:
+      long      |uv| f up to 1e5 lambda, sources 10-30 deg from the centre: |phase| 1e5 .. 1e6 rad
+      centre    one source exactly at the phase centre, rows 0-3 with u = v = w = 0 (the G == 0 branch)
+      widefd    a 40 MHz smearing width: the sinc far from 1 (and through its zeros)
+      tinyfd    a 1 Hz smearing width
+      gauss     Gaussians of extent 0, 1e-12 rad and of 1 rad (vanishing to underflow), both projections
+      bessel    disks and rings sized so that rows sit on zeros of j1 and j0
+      spectral  negative and zero Stokes fluxes, channels at f0 / 2, f0, 2 f0"""
+    b = small_problem(N=6, M=2, tilesz=4, seed=seed)
+    pr = b.pr
+    u, v, w = pr.u.copy(), pr.v.copy(), pr.w.copy()
+    rng = np.random.default_rng(seed + 1)
+    freqs = np.array([140e6, 150e6, 163e6])
+    fdelta = 195.3e3
+    K = 8
+
+    def cluster(ll, mm, sI, stype=None, **kw):
+        ll, mm = np.asarray(ll, dtype=np.float64), np.asarray(mm, dtype=np.float64)
+        n = len(ll)
+        sI = np.asarray(sI, dtype=np.float64)
+        cl = dict(ll=ll, mm=mm, nn=np.sqrt(1.0 - ll * ll - mm * mm) - 1.0, sI=sI,
+                  sQ=0.3 * sI * rng.uniform(-1, 1, n), sU=0.2 * sI * rng.uniform(-1, 1, n),
+                  sV=0.05 * sI * rng.uniform(-1, 1, n),
+                  stype=np.zeros(n, dtype=np.uint8) if stype is None else np.asarray(stype, np.uint8))
+        cl.update(kw)
+        return cl
+
+    def around(lo_deg, hi_deg, n):
+        r = np.deg2rad(rng.uniform(lo_deg, hi_deg, n))
+        a = rng.uniform(0, 2 * np.pi, n)
+        return np.sin(r) * np.cos(a), np.sin(r) * np.sin(a)
+
+    def gauss_tab(eX, eY, proj):
+        g = np.zeros((len(eX), 8))
+        xi, ph = rng.uniform(0, 2 * np.pi, len(eX)), rng.uniform(0, 0.4, len(eX))
+        g[:, 0], g[:, 1], g[:, 2] = eX, eY, rng.uniform(0, np.pi, len(eX))
+        g[:, 3], g[:, 4], g[:, 5], g[:, 6], g[:, 7] = np.cos(xi), np.sin(xi), np.cos(ph), np.sin(ph), proj
+        return g
+
+    if name == "long":
+        s = 1e5 / (np.max(np.hypot(u, v)) * freqs[-1])
+        u, v, w = u * s, v * s, w * s
+        l, m = around(10, 30, K)
+        st = np.array([0, 0, 0, 1, 0, 1, 0, 0], dtype=np.uint8)
+        g = gauss_tab(np.full(K, 1e-7), np.full(K, 2e-7), np.arange(K) % 2)
+        cls = [cluster(l[:5], m[:5], rng.lognormal(0, 1, 5), st[:5], gauss=g[:5]),
+               cluster(l[5:], m[5:], rng.lognormal(0, 1, 3), st[5:], gauss=g[5:])]
+    elif name == "centre":
+        u[:4] = v[:4] = w[:4] = 0.0
+        l, m = around(0.5, 4, K)
+        l[0] = m[0] = 0.0
+        st = np.array([0, 1, 0, 1, 0, 0, 0, 0], dtype=np.uint8)
+        g = gauss_tab(np.full(K, 3e-4), np.full(K, 1e-4), np.arange(K) % 2)
+        cls = [cluster(l[:4], m[:4], rng.lognormal(0, 1, 4), st[:4], gauss=g[:4]),
+               cluster(l[4:], m[4:], rng.lognormal(0, 1, 4), st[4:], gauss=g[4:])]
+    elif name in ("widefd", "tinyfd"):
+        fdelta = 40e6 if name == "widefd" else 1.0
+        l, m = around(1, 8, K)
+        cls = [cluster(l[:4], m[:4], rng.lognormal(0, 1, 4)), cluster(l[4:], m[4:], rng.lognormal(0, 1, 4))]
+    elif name == "gauss":
+        l, m = around(0.5, 4, K)
+        eX = np.array([0.0, 1e-12, 1.0, 1.0, 2e-4, 1e-12, 0.7, 3e-4])
+        eY = np.array([0.0, 3e-12, 1.0, 0.5, 1e-4, 1e-12, 1.2, 0.0])
+        g = gauss_tab(eX, eY, np.arange(K) % 2)
+        cls = [cluster(l[:4], m[:4], rng.lognormal(0, 1, 4), np.ones(4), gauss=g[:4]),
+               cluster(l[4:], m[4:], rng.lognormal(0, 1, 4), np.ones(4), gauss=g[4:])]
+    elif name == "bessel":
+        from scipy import special
+        l, m = around(0.5, 4, K)
+        st = np.array([2, 2, 2, 3, 3, 3, 2, 3], dtype=np.uint8)
+        zeros = {2: special.jn_zeros(1, 3), 3: special.jn_zeros(0, 3)}
+        disk = {}
+        rows = rng.choice(np.arange(4, len(u)), K, replace=False)
+        for s in range(K):
+            xi, ph = rng.uniform(0, 2 * np.pi), rng.uniform(0, 0.4)
+            cxi, sxi, cph, sph = np.cos(xi), np.sin(xi), np.cos(ph), np.sin(ph)
+            r, f = rows[s], freqs[0]
+            up = u[r] * f * cxi - v[r] * f * cph * sxi + w[r] * f * sph * sxi
+            vp = u[r] * f * sxi + v[r] * f * cph * cxi - w[r] * f * sph * cxi
+            eX = zeros[int(st[s])][s % 3] / (2.0 * np.pi * np.hypot(up, vp))
+            disk[s] = (eX, cxi, sxi, cph, sph, 1)
+        cls = [cluster(l[:4], m[:4], rng.lognormal(0, 1, 4), st[:4], disk={s: disk[s] for s in range(4)}),
+               cluster(l[4:], m[4:], rng.lognormal(0, 1, 4), st[4:],
+                       disk={s - 4: disk[s] for s in range(4, K)})]
+    elif name == "spectral":
+        freqs = np.array([75e6, 150e6, 300e6])
+        l, m = around(0.5, 4, K)
+        sI0 = np.array([1.5, -2.0, 0.0, 0.8, -0.3, 2.2, 1.0, 0.6])
+        sQ0 = np.array([0.0, 0.4, -0.1, 0.0, 0.2, -0.5, 0.0, 0.1])
+        sU0 = np.array([-0.2, 0.0, 0.3, 0.1, 0.0, 0.0, -0.4, 0.0])
+        sV0 = np.array([0.05, -0.01, 0.0, 0.0, 0.02, 0.0, 0.0, -0.03])
+        spec = dict(sI0=sI0, sQ0=sQ0, sU0=sU0, sV0=sV0,
+                    f0=np.array([150e6, 150e6, 75e6, 300e6, 150e6, 150e6, 140e6, 150e6]),
+                    spec_idx=np.array([-0.7, 0.9, -0.7, 0.0, 1.3, -2.1, 0.0, -0.8]),
+                    spec_idx1=np.array([0.05, -0.2, 0.0, 0.3, 0.1, 0.0, 0.4, -0.1]),
+                    spec_idx2=np.array([-0.01, 0.03, 0.2, 0.0, 0.0, -0.05, 0.0, 0.02]))
+        cls = []
+        for a, z in ((0, 4), (4, 8)):
+            cl = cluster(l[a:z], m[a:z], 0.9 * sI0[a:z] + 0.05)
+            cl.update({kk: vv[a:z] for kk, vv in spec.items()})
+            cls.append(cl)
+    else:
+        raise ValueError(name)
+    return u, v, w, cls, freqs, fdelta
+
+
+SKY_EDGE_CASES = ["long", "centre", "widefd", "tinyfd", "gauss", "bessel", "spectral"]
+
+
 def lsum(a):
     """sum in long double (scalar references of the device reductions)"""
     return float(np.sum(np.asarray(a, dtype=np.longdouble)))
