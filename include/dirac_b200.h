@@ -527,4 +527,6 @@ int dirac_b200_bigtri_solve(int n, const double *L, const double *b, double *x, 
 
 /* simulation with solutions (predict_visibilities_multifreq_withsol and its beam variants) */
 #include "dirac_b200_withsol.h"
+/* coherencies of the diffuse cluster from a spatial model (recalculate_diffuse_coherencies) */
+#include "dirac_b200_diffuse.h"
 #endif

@@ -85,7 +85,36 @@ struct BeamArgs {
   double2 *E;                    // out, or null
 };
 
+// diffuse cluster (recalculate_diffuse_coherencies, diffuse_predict.c:295-586; kernels_diffuse.cu)
+struct DiffuseSource {
+  double ll, mm, nn, beta;   // direction; shapelet scale in the Fourier plane (exinfo_shapelet.beta)
+  int n0, pad_;
+  long long scoh;            // first entry in DiffuseArgs::scoh ([n0*n0][4] Stokes-weighted modes)
+  long long cf1, cf2;        // first entries of its two product tensors in DiffuseArgs::cf
+  long long cjq;             // first entry of its station products in DiffuseArgs::cjq ([N][n0*n0][4])
+};
+struct DiffuseArgs {
+  const DiffuseSource *src;
+  int ns;                    // sources, in the reference's order
+  int N, sh;                 // stations; order of the spatial model (G = sh*sh modes)
+  const double2 *Zt;         // [N][G][4] per-station spatial modes, 2x2 blocks transposed (:374-383)
+  const double2 *scoh;
+  const double *cf;
+  double2 *cjq;              // scratch: C_Jq of every source and station
+  const short2 *pairs;       // [npairs] stations (p, q) of each baseline
+  int npairs;
+  const long long *row_off;  // [npairs + 1] rows of baseline b: rows[row_off[b] .. row_off[b+1])
+  const long long *rows;     //   or, when null, rows b + t*Nbase, t < ntime
+  int ntime, Nbase;
+  const double *u, *v, *w;   // [R] seconds
+  double freq0, fdelta2;
+  long long R;
+  double2 *coh;              // planar [4][R] of the cluster, rewritten
+};
+
 extern "C" {
+// station products, then the prediction of every row (profile kind 12); max_n0: largest source order
+void db_launch_diffuse(const DiffuseArgs *a, int max_n0, cudaStream_t st);
 void db_launch_coherencies(const CohArgs *a, cudaStream_t st);
 void db_launch_predict_multifreq(const CohArgs *a, cudaStream_t st);
 void db_launch_residual_multifreq(const CohArgs *a, cudaStream_t st);

@@ -15,11 +15,41 @@
 #endif
 
 // ---- per-source term ------------------------------------------------------------------------------
+// bb[n] = phi_n(x) = H_n(x) exp(-x^2/2) / sqrt(2^(n+1) n!), n < n0 (calculate_uv_mode_vectors_scalar,
+// shapelet.c:84-95): the recursion of shapelet_factor below, for the diffuse cluster's rows
+// (diffuse_math.cuh).  shapelet_factor keeps its own copy: routed through this helper, nvcc schedules
+// the sky-prediction kernel differently.
+__host__ __device__ __forceinline__ void shapelet_basis(double x, int n0, double *bb) {
+  const double ex = exp(-0.5 * x * x);
+  double hm2 = 1.0, hm1 = 2.0 * x, fact = 1.0, p2 = 2.0;  // H_0, H_1, n!, 2^(n+1)
+  for (int n = 0; n < n0; n++) {
+    double h;
+    if (n == 0) h = 1.0;
+    else if (n == 1) h = hm1;
+    else {
+      h = 2.0 * x * hm1 - 2.0 * (double)(n - 1) * hm2;
+      hm2 = hm1;
+      hm1 = h;
+    }
+    if (n > 0) fact *= (double)n;
+    bb[n] = h * ex / sqrt(p2 * fact);
+    p2 *= 2.0;
+  }
+}
+// mode vector entry of mode (n1, n2): sign * phi_n1(-u beta) phi_n2(v beta); *odd: the mode is
+// imaginary (calculate_uv_mode_vectors_scalar, shapelet.c:109-127)
+__host__ __device__ __forceinline__ double shapelet_mode_coeff(const double *bu, const double *bv, int n1,
+                                                      int n2, int *odd) {
+  *odd = (n1 + n2) & 1;
+  const int sg = (((n1 + n2 - *odd) / 2) & 1) ? -1 : 1;
+  return (sg < 0 ? -bu[n1] : bu[n1]) * bv[n2];
+}
+
 // phase * |sinc| smearing * shape factor for one source at one frequency (predict.c:411-470)
 // Fourier-plane value of a shapelet source (shapelet_contrib + calculate_uv_mode_vectors_scalar,
 // shapelet.c:50-190): sum over the n0 x n0 modes of coeff * phi_n1(-ut beta) phi_n2(vt beta), odd
 // n1+n2 imaginary, phi_n(x) = H_n(x) exp(-x^2/2) / sqrt(2^(n+1) n!), times 2 pi / (eX eY)
-__host__ __device__ __noinline__ double2 shapelet_factor(const DevSource &s, const double *modes, double uf,
+static __host__ __device__ __noinline__ double2 shapelet_factor(const DevSource &s, const double *modes, double uf,
                                                 double vf, double wf) {
   double up, vp;
   if (s.use_projection != 0.0) {

@@ -24,12 +24,12 @@ static cudaEvent_t prof_event() {
   DB_CHECK(cudaEventCreate(&e));
   return e;
 }
-static unsigned long long g_kind_count[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+static unsigned long long g_kind_count[13] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 extern "C" unsigned long long dirac_b200_kernel_count(int kind) {
-  return (kind >= 0 && kind < 12) ? g_kind_count[kind] : 0ull;
+  return (kind >= 0 && kind < 13) ? g_kind_count[kind] : 0ull;
 }
 void db_prof_begin(int kind, double bytes, cudaStream_t st) {
-  if (kind >= 0 && kind < 12) g_kind_count[kind]++;
+  if (kind >= 0 && kind < 13) g_kind_count[kind]++;
   if (!g_prof_on) return;
   ProfRec r; r.a = prof_event(); r.b = prof_event(); r.kind = kind; r.bytes = bytes;
   DB_CHECK(cudaEventRecord(r.a, st));

@@ -324,6 +324,23 @@ class DiracAPI:
             tilesz, barr, sky.arr, sky.M, dptr(freqs), len(freqs), fdelta, tdelta, dec0, Nt,
             add_to_data, ccid, rho, phase_only)
 
+    def recalculate_diffuse_coherencies(self, u, v, w, x, N, barr, sky: SkyModel, freq0, fdelta, cid,
+                                        sh_n0, sh_beta, Z, tdelta=10.0, dec0=1.0, uvmin=0.0,
+                                        uvmax=1e9, Nt=4, use_cuda=0):
+        """coherencies of cluster cid rewritten from the spatial model Z (Dirac_radio.h:228).
+        x: [row][M][4] complex, in/out (only cluster cid changes); Z: 2N x 2G complex (G = sh_n0^2),
+        passed column major"""
+        L = self.lib
+        L.recalculate_diffuse_coherencies.restype = C.c_int
+        L.recalculate_diffuse_coherencies.argtypes = [
+            c_double_p, c_double_p, c_double_p, c_double_p, C.c_int, C.c_int, C.POINTER(baseline_t),
+            C.POINTER(clus_source_t), C.c_int, C.c_double, C.c_double, C.c_double, C.c_double,
+            C.c_double, C.c_double, C.c_int, C.c_int, C.c_double, c_double_p, C.c_int, C.c_int]
+        Zf = np.asfortranarray(Z, dtype=np.complex128).reshape(-1, order="F")
+        return L.recalculate_diffuse_coherencies(
+            dptr(u), dptr(v), dptr(w), cptr(x), N, len(u), barr, sky.arr, sky.M, freq0, fdelta,
+            tdelta, dec0, uvmin, uvmax, cid, sh_n0, sh_beta, cptr(Zf), Nt, use_cuda)
+
     # ---- station beams (Dirac_radio.h:472-490) ----
     def precalculate_coherencies_withbeam(self, u, v, w, N, Nbase1, barr, sky, freq0, fdelta, beam,
                                           tdelta=10.0, dec0=1.0, uvmin=0.0, uvmax=1e9, Nt=4):

@@ -46,6 +46,9 @@ WITHSOL_EXPORTED = [
     "predict_visibilities_withsol_withbeam_gpu",
 ]
 
+#: every symbol include/dirac_b200_diffuse.h declares (diffuse cluster from a spatial model)
+DIFFUSE_EXPORTED = ["recalculate_diffuse_coherencies", "dirac_b200_diffuse_coherencies"]
+
 
 class DiracB200(DiracAPI):
     """The product library: the reference entry points (inherited bindings) plus the thin
@@ -204,6 +207,18 @@ class DeviceProblem:
     def precalculate(self, u, v, w, freq0, fdelta, uvmin=0.0, uvmax=1e9, barr=None):
         self.api.lib.dirac_b200_precalculate(self.h, dptr(u), dptr(v), dptr(w), self.sky.arr,
                                              freq0, fdelta, uvmin, uvmax, barr)
+
+    def diffuse_coherencies(self, u, v, w, freq0, fdelta, cid, sh_n0, sh_beta, Z):
+        """dirac_b200_diffuse_coherencies: rewrite local cluster cid's resident coherencies from the
+        spatial model Z (2N x 2G complex, column major, G = sh_n0^2)"""
+        L = self.api.lib
+        L.dirac_b200_diffuse_coherencies.restype = C.c_int
+        L.dirac_b200_diffuse_coherencies.argtypes = [C.c_void_p, c_double_p, c_double_p, c_double_p,
+                                                     C.POINTER(clus_source_t), C.c_double, C.c_double,
+                                                     C.c_int, C.c_int, C.c_double, c_double_p]
+        Zf = np.asfortranarray(Z, dtype=np.complex128).reshape(-1, order="F")
+        return L.dirac_b200_diffuse_coherencies(self.h, dptr(u), dptr(v), dptr(w), self.sky.arr, freq0,
+                                                fdelta, cid, sh_n0, sh_beta, cptr(Zf))
 
     def get_coherencies(self):
         coh = np.zeros(4 * self.sky.M * self.Nbase * self.tilesz, dtype=np.complex128)
