@@ -529,4 +529,6 @@ int dirac_b200_bigtri_solve(int n, const double *L, const double *b, double *x, 
 #include "dirac_b200_withsol.h"
 /* coherencies of the diffuse cluster from a spatial model (recalculate_diffuse_coherencies) */
 #include "dirac_b200_diffuse.h"
+/* per-channel refinement (calculate_residuals and the channel loop on one resident problem) */
+#include "dirac_b200_channels.h"
 #endif

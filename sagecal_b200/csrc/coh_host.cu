@@ -5,6 +5,7 @@
 #include <vector>
 
 #include "../../include/dirac_b200.h"
+#include "../../include/dirac_b200_channels.h"
 #include "coh.h"
 #include "problem.h"
 
@@ -92,6 +93,7 @@ static void sky_upload(const clus_source_t *carr, int M, SkyDev *sky, cudaStream
   db_stream_sync(st);  // the vectors go out of scope
   sky->nseg = (int)segs.size();
   sky->nsrc = (int)src.size();
+  db_count_sky_upload();
 }
 
 static void sky_free(SkyDev *sky) {
@@ -307,6 +309,7 @@ static int precalculate_impl(double *u, double *v, double *w, double *x, int N, 
   DB_CHECK(cudaMemcpyAsync(hf.data(), dflag, R, cudaMemcpyDeviceToHost, st));
   db_stream_sync(st);
   DB_CHECK(cudaGetLastError());
+  db_count_coh_host_bytes((size_t)R * M * 64);
   for (long long r = 0; r < R; r++) barr[r].flag = hf[r];
   cudaFree(stage); cudaFree(dcoh); cudaFree(dflag);
   cudaFree(du); cudaFree(dv); cudaFree(dw); cudaFree(df);
@@ -631,6 +634,71 @@ extern "C" int dirac_b200_extract_phases(const double *p, double *pout, int N, i
   return 0;
 }
 
+// what MODE 2 of the sky kernel reads besides the sky: chunk tables, the stations of every row and the
+// sign of every cluster; cm: the LAST cluster with id == ccid (residual.c:584-590), or -1
+struct ResidualTables {
+  int *dn, *dc0, *dpo, *ds1, *ds2;
+  signed char *dcoef;
+  int cm;
+  long long npar;  // doubles of p the chunk offsets reach
+  void upload(const baseline_t *barr, const clus_source_t *carr, int N, int M, long long R,
+              const std::vector<signed char> &coef, int ccid, cudaStream_t st) {
+    std::vector<int> nchunk(M), chunk0(M), poff, s1(R), s2(R);
+    int mt = 0;
+    cm = -1;
+    npar = 0;
+    for (int k = 0; k < M; k++) {
+      nchunk[k] = carr[k].nchunk;
+      chunk0[k] = mt;
+      if (carr[k].id == ccid) cm = k;
+      for (int c = 0; c < carr[k].nchunk; c++) {
+        poff.push_back(carr[k].p[c]);
+        if ((long long)carr[k].p[c] + 8ll * N > npar) npar = (long long)carr[k].p[c] + 8ll * N;
+      }
+      mt += carr[k].nchunk;
+    }
+    for (long long r = 0; r < R; r++) {
+      s1[r] = barr[r].sta1;
+      s2[r] = barr[r].sta2;
+    }
+    DB_CHECK(cudaMalloc((void **)&dn, sizeof(int) * M));
+    DB_CHECK(cudaMalloc((void **)&dc0, sizeof(int) * M));
+    DB_CHECK(cudaMalloc((void **)&dpo, sizeof(int) * (mt > 0 ? mt : 1)));
+    DB_CHECK(cudaMalloc((void **)&ds1, sizeof(int) * R));
+    DB_CHECK(cudaMalloc((void **)&ds2, sizeof(int) * R));
+    DB_CHECK(cudaMalloc((void **)&dcoef, M));
+    DB_CHECK(cudaMemcpyAsync(dn, nchunk.data(), sizeof(int) * M, cudaMemcpyHostToDevice, st));
+    DB_CHECK(cudaMemcpyAsync(dc0, chunk0.data(), sizeof(int) * M, cudaMemcpyHostToDevice, st));
+    DB_CHECK(cudaMemcpyAsync(dpo, poff.data(), sizeof(int) * mt, cudaMemcpyHostToDevice, st));
+    DB_CHECK(cudaMemcpyAsync(ds1, s1.data(), sizeof(int) * R, cudaMemcpyHostToDevice, st));
+    DB_CHECK(cudaMemcpyAsync(ds2, s2.data(), sizeof(int) * R, cudaMemcpyHostToDevice, st));
+    DB_CHECK(cudaMemcpyAsync(dcoef, coef.data(), M, cudaMemcpyHostToDevice, st));
+    db_stream_sync(st);  // the vectors go out of scope
+  }
+  void point(CohArgs *a) const {
+    a->sta1 = ds1; a->sta2 = ds2; a->clus_nchunk = dn; a->clus_chunk0 = dc0; a->chunk_poff = dpo;
+    a->clus_coef = dcoef;
+  }
+  void free() {
+    cudaFree(dn); cudaFree(dc0); cudaFree(dpo); cudaFree(ds1); cudaFree(ds2); cudaFree(dcoef);
+  }
+};
+// (J + rho I)^-1 of every station and chunk of the correction cluster, [nchunk][N][8]; phase_only: of
+// the phases of its jointly diagonalised solutions (residual.c:975-990)
+static void correction_inverse(const double *p, const clus_source_t &c, int N, double rho,
+                               int phase_only, std::vector<double> &pinv) {
+  pinv.resize((size_t)8 * N * c.nchunk);
+  std::vector<double> pphase(phase_only ? (size_t)8 * N : 0);
+  for (int ck = 0; ck < c.nchunk; ck++) {
+    const double *pm = p + c.p[ck];
+    if (phase_only) {
+      extract_phases_host(pm, pphase.data(), N, 10);
+      pm = pphase.data();
+    }
+    for (int s = 0; s < N; s++) jones_invert(pm + 8 * s, pinv.data() + (size_t)8 * N * ck + 8 * s, rho);
+  }
+}
+
 // Dirac_radio.h:652,666 (residual.c:940-1061,1620-1740): the model of every cluster with the solved
 // Jones, per channel, x[chan][row][8] += coef[k] J_p C_k(chan) J_q^H (coef -1, 0 or +1 per cluster;
 // clear_x: x starts from zero instead of the caller's data), the coherencies re-predicted from the
@@ -655,53 +723,12 @@ static int residuals_multifreq_impl(double *u, double *v, double *w, double *p, 
   sky_upload(carr, M, &sky, st);
   double *du = upload_doubles(u, R, st), *dv = upload_doubles(v, R, st);
   double *dw = upload_doubles(w, R, st), *df = upload_doubles(freqs, Nchan, st);
-  // cluster / chunk tables, stations, solutions
-  std::vector<int> nchunk(M), chunk0(M), poff, s1(R), s2(R);
-  int mt = 0, cm = -1;
-  long long npar = 0;
-  for (int k = 0; k < M; k++) {
-    nchunk[k] = carr[k].nchunk;
-    chunk0[k] = mt;
-    if (carr[k].id == ccid) cm = k;
-    for (int c = 0; c < carr[k].nchunk; c++) {
-      poff.push_back(carr[k].p[c]);
-      if ((long long)carr[k].p[c] + 8ll * N > npar) npar = (long long)carr[k].p[c] + 8ll * N;
-    }
-    mt += carr[k].nchunk;
-  }
-  for (long long r = 0; r < R; r++) {
-    s1[r] = barr[r].sta1;
-    s2[r] = barr[r].sta2;
-  }
+  ResidualTables tb;
+  tb.upload(barr, carr, N, M, R, coef, ccid, st);
+  const int cm = tb.cm;
   std::vector<double> pinv;
-  if (cm >= 0) {
-    pinv.resize((size_t)8 * N * carr[cm].nchunk);
-    std::vector<double> pphase(phase_only ? (size_t)8 * N : 0);
-    for (int c = 0; c < carr[cm].nchunk; c++) {
-      const double *pm = p + carr[cm].p[c];
-      if (phase_only) {  // only the phases of the jointly diagonalised solutions (residual.c:975-990)
-        extract_phases_host(pm, pphase.data(), N, 10);
-        pm = pphase.data();
-      }
-      for (int s = 0; s < N; s++)
-        jones_invert(pm + 8 * s, pinv.data() + (size_t)8 * N * c + 8 * s, rho);
-    }
-  }
-  int *dn = nullptr, *dc0 = nullptr, *dpo = nullptr, *ds1 = nullptr, *ds2 = nullptr;
-  signed char *dcoef = nullptr;
-  DB_CHECK(cudaMalloc((void **)&dn, sizeof(int) * M));
-  DB_CHECK(cudaMalloc((void **)&dc0, sizeof(int) * M));
-  DB_CHECK(cudaMalloc((void **)&dpo, sizeof(int) * (mt > 0 ? mt : 1)));
-  DB_CHECK(cudaMalloc((void **)&ds1, sizeof(int) * R));
-  DB_CHECK(cudaMalloc((void **)&ds2, sizeof(int) * R));
-  DB_CHECK(cudaMalloc((void **)&dcoef, M));
-  DB_CHECK(cudaMemcpyAsync(dn, nchunk.data(), sizeof(int) * M, cudaMemcpyHostToDevice, st));
-  DB_CHECK(cudaMemcpyAsync(dc0, chunk0.data(), sizeof(int) * M, cudaMemcpyHostToDevice, st));
-  DB_CHECK(cudaMemcpyAsync(dpo, poff.data(), sizeof(int) * mt, cudaMemcpyHostToDevice, st));
-  DB_CHECK(cudaMemcpyAsync(ds1, s1.data(), sizeof(int) * R, cudaMemcpyHostToDevice, st));
-  DB_CHECK(cudaMemcpyAsync(ds2, s2.data(), sizeof(int) * R, cudaMemcpyHostToDevice, st));
-  DB_CHECK(cudaMemcpyAsync(dcoef, coef.data(), M, cudaMemcpyHostToDevice, st));
-  double *dp = upload_doubles(p, npar, st);
+  if (cm >= 0) correction_inverse(p, carr[cm], N, rho, phase_only, pinv);
+  double *dp = upload_doubles(p, tb.npar, st);
   double *dpinv = cm >= 0 ? upload_doubles(pinv.data(), (long long)pinv.size(), st) : nullptr;
   double2 *dx = nullptr;
   const size_t nx = (size_t)Nchan * R * 4;
@@ -715,9 +742,9 @@ static int residuals_multifreq_impl(double *u, double *v, double *w, double *p, 
   memset(&a, 0, sizeof(a));
   a.u = du; a.v = dv; a.w = dw; a.src = sky.src; a.modes = sky.modes; a.segs = sky.segs; a.nseg = sky.nseg;
   a.freqs = df; a.Nchan = Nchan; a.fdelta2 = (fdelta / (double)Nchan) * 0.5;
-  a.R = R; a.xout = dx; a.sta1 = ds1; a.sta2 = ds2; a.p = dp; a.clus_nchunk = dn;
-  a.clus_chunk0 = dc0; a.chunk_poff = dpo; a.clus_coef = dcoef; a.pinv = dpinv;
+  a.R = R; a.xout = dx; a.p = dp; a.pinv = dpinv;
   a.pinv_nchunk = cm >= 0 ? carr[cm].nchunk : 1; a.N = N;
+  tb.point(&a);
   BeamDev bd;
   beam_prepare(beam, sky, N, Nbase, freqs, Nchan, df, barr, R, st, &a, &bd);
   db_prof_begin(11, 128.0 * (double)nx / 4.0, st);  // profile kind 11: x read and written once
@@ -729,7 +756,7 @@ static int residuals_multifreq_impl(double *u, double *v, double *w, double *p, 
   DB_CHECK(cudaGetLastError());
   cudaFree(dx); cudaFree(du); cudaFree(dv); cudaFree(dw); cudaFree(df); cudaFree(dp);
   if (dpinv) cudaFree(dpinv);
-  cudaFree(dn); cudaFree(dc0); cudaFree(dpo); cudaFree(ds1); cudaFree(ds2); cudaFree(dcoef);
+  tb.free();
   beam_free(&bd);
   sky_free(&sky);
   cudaStreamDestroy(st);
@@ -758,6 +785,92 @@ extern "C" int calculate_residuals_multifreq(double *u, double *v, double *w, do
   (void)tdelta; (void)dec0; (void)Nt;
   return residuals_multifreq_impl(u, v, w, p, x, N, Nbase, tilesz, barr, carr, M, freqs, Nchan, fdelta,
                                   residual_coef(carr, M), false, ccid, rho, phase_only, nullptr);
+}
+// Dirac_radio.h:639 (residual.c:314-674): one channel at freq0; the worker is the multi-channel one
+// with the channel loop taken out (no phase_only here)
+extern "C" int calculate_residuals(double *u, double *v, double *w, double *p, double *x, int N,
+                                   int Nbase, int tilesz, baseline_t *barr, clus_source_t *carr,
+                                   int M, double freq0, double fdelta, double tdelta, double dec0,
+                                   int Nt, int ccid, double rho) {
+  (void)tdelta; (void)dec0; (void)Nt;
+  return residuals_multifreq_impl(u, v, w, p, x, N, Nbase, tilesz, barr, carr, M, &freq0, 1, fdelta,
+                                  residual_coef(carr, M), false, ccid, rho, 0, nullptr);
+}
+
+// The per-channel refinement of one interval (driver option -b 1, fullbatch_mode.cpp:464-497) on ONE
+// resident problem.  Per channel: coherencies at the channel straight into the planar storage (with
+// the uv cut accumulating in the resident flags, predict.c:489-495), LBFGS from the start Jones, then
+// the residual re-predicted from the sky with the channel's spectral fluxes and the solved Jones, on
+// the channel's data kept in API layout on the device.  Only the data of a channel go up and its
+// residual comes down.
+extern "C" int dirac_b200_bfgsfit_channels(double *u, double *v, double *w, double *xo, int N,
+                                           int Nbase, int tilesz, baseline_t *barr,
+                                           clus_source_t *carr, int M, int Mt, double *freqs,
+                                           int Nchan, double deltafch, double uvmin, double uvmax,
+                                           double *p, int max_lbfgs, int lbfgs_m, int solver_mode,
+                                           double mean_nu, int ccid, double rho, double *res_00,
+                                           double *res_01, double *pfreq) {
+  if (Nchan < 1) return 0;
+  dirac_b200_problem *pr = dirac_b200_create(N, Nbase, tilesz, barr, carr, M, Mt, nullptr, nullptr);
+  DevProblem &d = pr->d;
+  cudaStream_t st = d.stream;
+  const long long R = d.R;
+  const size_t m = (size_t)8 * N * Mt;
+  SkyDev sky;
+  sky_upload(carr, M, &sky, st);
+  double *du = upload_doubles(u, R, st), *dv = upload_doubles(v, R, st);
+  double *dw = upload_doubles(w, R, st), *df = upload_doubles(freqs, Nchan, st);
+  ResidualTables tb;
+  tb.upload(barr, carr, N, M, R, residual_coef(carr, M), ccid, st);
+  std::vector<double> pinv, pown(pfreq ? 0 : m);
+  double *dpinv = nullptr;
+  if (tb.cm >= 0) DB_CHECK(cudaMalloc((void **)&dpinv, sizeof(double) * 8 * N * carr[tb.cm].nchunk));
+  double2 *dx = (double2 *)db_malloc(sizeof(double2) * 4 * (size_t)R);  // [R][4]: data in, residual out
+  CohArgs a;
+  memset(&a, 0, sizeof(a));
+  a.u = du; a.v = dv; a.w = dw; a.src = sky.src; a.modes = sky.modes; a.segs = sky.segs; a.nseg = sky.nseg;
+  a.Nchan = 1; a.fdelta2 = deltafch * 0.5; a.uvmin = uvmin; a.uvmax = uvmax; a.R = R; a.N = N;
+  a.pinv_nchunk = tb.cm >= 0 ? carr[tb.cm].nchunk : 1;
+  tb.point(&a);
+  double *pc = pown.data();
+  for (int ci = 0; ci < Nchan; ci++) {
+    double *xc = xo + (size_t)ci * 8 * R;
+    DB_CHECK(cudaMemcpyAsync(dx, xc, (size_t)R * 64, cudaMemcpyHostToDevice, st));
+    db_launch_vis_to_planar(dx, d.x, R, st);
+    a.freqs = df + ci;
+    a.coh = d.coh; a.flag = d.flag; a.xout = nullptr; a.p = nullptr; a.pinv = nullptr;
+    db_launch_coherencies(&a, st);
+    db_count_launch(2);
+    if (pfreq) pc = pfreq + (size_t)ci * m;
+    memcpy(pc, p, sizeof(double) * m);
+    db_bfgsfit_dev(pr, pc, max_lbfgs, lbfgs_m, solver_mode, mean_nu, res_00 + ci, res_01 + ci, false);
+    // the fit left the solution in d.pp
+    if (tb.cm >= 0) {
+      correction_inverse(pc, carr[tb.cm], N, rho, 0, pinv);
+      DB_CHECK(cudaMemcpyAsync(dpinv, pinv.data(), sizeof(double) * pinv.size(),
+                               cudaMemcpyHostToDevice, st));
+    }
+    a.coh = nullptr; a.flag = nullptr; a.xout = dx; a.p = d.pp; a.pinv = dpinv;
+    db_prof_begin(11, 128.0 * (double)R, st);
+    db_launch_residual_multifreq(&a, st);
+    db_prof_end(st);
+    db_count_launch(1);
+    DB_CHECK(cudaMemcpyAsync(xc, dx, (size_t)R * 64, cudaMemcpyDeviceToHost, st));
+    db_stream_sync(st);  // pinv is rewritten by the next channel
+  }
+  memcpy(p, pc, sizeof(double) * m);
+  std::vector<unsigned char> hf(R);
+  DB_CHECK(cudaMemcpyAsync(hf.data(), d.flag, R, cudaMemcpyDeviceToHost, st));
+  db_stream_sync(st);
+  DB_CHECK(cudaGetLastError());
+  for (long long r = 0; r < R; r++) barr[r].flag = hf[r];
+  db_free(dx);
+  if (dpinv) cudaFree(dpinv);
+  tb.free();
+  cudaFree(du); cudaFree(dv); cudaFree(dw); cudaFree(df);
+  sky_free(&sky);
+  dirac_b200_destroy(pr);
+  return 0;
 }
 // Dirac_radio.h:666 (residual.c:1620-1740): simulation with solutions
 extern "C" int predict_visibilities_multifreq_withsol(double *u, double *v, double *w, double *p,

@@ -10,6 +10,16 @@
 #include "problem.h"
 
 static unsigned long long g_launches = 0;
+// host <-> device traffic of the two large operands a resident call keeps on the device
+static unsigned long long g_sky_uploads = 0, g_coh_host_bytes = 0;
+void db_count_sky_upload() { g_sky_uploads++; }
+void db_count_coh_host_bytes(size_t bytes) { g_coh_host_bytes += bytes; }
+extern "C" void dirac_b200_transfer_stats(unsigned long long *sky_uploads,
+                                          unsigned long long *coh_host_bytes, int reset) {
+  if (sky_uploads) *sky_uploads = g_sky_uploads;
+  if (coh_host_bytes) *coh_host_bytes = g_coh_host_bytes;
+  if (reset) g_sky_uploads = g_coh_host_bytes = 0;
+}
 void db_count_launch(int n) { g_launches += (unsigned long long)n; }
 extern "C" unsigned long long dirac_b200_launch_count(void) { return g_launches; }
 
@@ -358,6 +368,7 @@ static dirac_b200_problem *create_impl(int N, int Nbase, int tilesz, const basel
       db_launch_coh_to_planar(stage, d.coh, r0, nr, M, R, d.stream);
       db_count_launch(1);
     }
+    db_count_coh_host_bytes((size_t)R * M * 64);
     db_stream_sync(d.stream);
     db_free(stage);
   }
@@ -433,6 +444,7 @@ extern "C" void dirac_b200_get_coherencies(dirac_b200_problem *pr, double *coh) 
                              cudaMemcpyDeviceToHost, d.stream));
   }
   db_stream_sync(d.stream);
+  db_count_coh_host_bytes((size_t)d.R * d.M * 64);
   db_free(stage);
 }
 

@@ -105,6 +105,12 @@ double db_cost_window_dev(dirac_b200_problem *pr, const double *pp_dev, double2 
                           long long r_lo, long long r_hi);
 void db_grad_window_dev(dirac_b200_problem *pr, const double *pp_dev, double *g_dev, double nu,
                         long long r_lo, long long r_hi);
+// bfgsfit_visibilities on a resident problem (sage.cu)
+int db_bfgsfit_dev(dirac_b200_problem *pr, double *pp, int max_lbfgs, int lbfgs_m, int solver_mode,
+                   double mean_nu, double *res_0, double *res_1, bool keep_residual);
+// sky models uploaded / bytes of coherencies copied between host and device (dirac_b200_transfer_stats)
+void db_count_sky_upload();
+void db_count_coh_host_bytes(size_t bytes);
 void db_lm_init(dirac_b200_problem *pr);
 void db_prefactor_sweep(dirac_b200_problem *pr, double tau);
 void db_allreduce(dirac_b200_problem *pr, void *dev, long long count);

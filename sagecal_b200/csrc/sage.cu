@@ -298,17 +298,14 @@ SAGEFIT_ALIAS(sagefit_visibilities_dual_pt_flt)
 SAGEFIT_ALIAS(sagefit_visibilities_dual_pt)
 SAGEFIT_ALIAS(sagefit_visibilities_dual_pt_one_gpu)
 
-extern "C" int bfgsfit_visibilities(double *u, double *v, double *w, double *x, int N, int Nbase,
-                                    int tilesz, baseline_t *barr, clus_source_t *carr,
-                                    double *coh, int M, int Mt, double freq0, double fdelta,
-                                    double *pp, double uvmin, int Nt, int max_lbfgs, int lbfgs_m,
-                                    int gpu_threads, int solver_mode, double mean_nu,
-                                    double *res_0, double *res_1) {
-  (void)u; (void)v; (void)w; (void)freq0; (void)fdelta; (void)uvmin; (void)Nt; (void)gpu_threads;
-  const int m = N * Mt * 8;
-  const long long n = (long long)Nbase * tilesz * 8;
-  dirac_b200_problem *pr = dirac_b200_create(N, Nbase, tilesz, barr, carr, M, Mt, coh, x);
+// LBFGS over all clusters on a resident problem, as bfgsfit_visibilities runs it (lmfit.c:1056-1180):
+// pp host, in/out; the cost before and after; the residual at the solution goes to pr->res only when
+// keep_residual (a caller that forms its own residual spares the store)
+int db_bfgsfit_dev(dirac_b200_problem *pr, double *pp, int max_lbfgs, int lbfgs_m, int solver_mode,
+                   double mean_nu, double *res_0, double *res_1, bool keep_residual) {
   DevProblem &d = pr->d;
+  const int m = d.N * d.Mt * 8;
+  const long long n = (long long)d.Nbase * d.tilesz * 8;
   DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * m, cudaMemcpyHostToDevice, d.stream));
   db_predict_dev(pr, d.pp, nullptr, 0, 1, 0.0, 0);
   *res_0 = sqrt(db_read_scalar(pr, 0)) / (double)n;
@@ -321,12 +318,24 @@ extern "C" int bfgsfit_visibilities(double *u, double *v, double *w, double *x, 
     }
   }
   DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * m, cudaMemcpyHostToDevice, d.stream));
-  db_predict_dev(pr, d.pp, pr->res, 1, 1, 0.0, 0);
+  db_predict_dev(pr, d.pp, keep_residual ? pr->res : nullptr, keep_residual ? 1 : 0, 1, 0.0, 0);
   *res_1 = sqrt(db_read_scalar(pr, 0)) / (double)n;
+  return (*res_1 > *res_0) ? -1 : 0;
+}
+
+extern "C" int bfgsfit_visibilities(double *u, double *v, double *w, double *x, int N, int Nbase,
+                                    int tilesz, baseline_t *barr, clus_source_t *carr,
+                                    double *coh, int M, int Mt, double freq0, double fdelta,
+                                    double *pp, double uvmin, int Nt, int max_lbfgs, int lbfgs_m,
+                                    int gpu_threads, int solver_mode, double mean_nu,
+                                    double *res_0, double *res_1) {
+  (void)u; (void)v; (void)w; (void)freq0; (void)fdelta; (void)uvmin; (void)Nt; (void)gpu_threads;
+  dirac_b200_problem *pr = dirac_b200_create(N, Nbase, tilesz, barr, carr, M, Mt, coh, x);
+  const int rv = db_bfgsfit_dev(pr, pp, max_lbfgs, lbfgs_m, solver_mode, mean_nu, res_0, res_1, true);
   db_download_vis(pr, pr->res, x);
   DB_CHECK(cudaGetLastError());
   dirac_b200_destroy(pr);
-  return (*res_1 > *res_0) ? -1 : 0;
+  return rv;
 }
 
 extern "C" int bfgsfit_visibilities_gpu(double *u, double *v, double *w, double *x, int N,

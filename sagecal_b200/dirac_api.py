@@ -324,6 +324,42 @@ class DiracAPI:
             tilesz, barr, sky.arr, sky.M, dptr(freqs), len(freqs), fdelta, tdelta, dec0, Nt,
             add_to_data, ccid, rho, phase_only)
 
+    def calculate_residuals(self, u, v, w, p, x, N, Nbase, tilesz, barr, sky: SkyModel, freq0, fdelta,
+                            tdelta=10.0, dec0=1.0, Nt=4, ccid=-99999, rho=1e-9):
+        """single-channel residual (Dirac_radio.h:639).  x[row][8]: data in, residual (optionally
+        corrected by cluster `ccid`) out"""
+        L = self.lib
+        L.calculate_residuals.restype = C.c_int
+        L.calculate_residuals.argtypes = [c_double_p] * 5 + [C.c_int] * 3 + [
+            C.POINTER(baseline_t), C.POINTER(clus_source_t), C.c_int] + [C.c_double] * 4 + [
+            C.c_int, C.c_int, C.c_double]
+        return L.calculate_residuals(dptr(u), dptr(v), dptr(w), dptr(p), dptr(x), N, Nbase, tilesz,
+                                     barr, sky.arr, sky.M, freq0, fdelta, tdelta, dec0, Nt, ccid, rho)
+
+    def bfgsfit_channels(self, u, v, w, xo, N, Nbase, tilesz, barr, sky: SkyModel, freqs, deltafch, p,
+                         uvmin=0.0, uvmax=1e9, max_lbfgs=10, lbfgs_m=7, solver_mode=SM_LM_LBFGS,
+                         mean_nu=2.0, ccid=-99999, rho=1e-9, keep_pfreq=True):
+        """dirac_b200_bfgsfit_channels: the per-channel refinement of one interval on a resident
+        problem.  xo [Nchan][row][8] data -> residual, p start Jones -> last channel's solution,
+        barr flags updated by the uv cut of every channel.
+        returns (retval, res_00 [Nchan], res_01 [Nchan], pfreq [Nchan, 8 N Mt] or None)"""
+        L = self.lib
+        L.dirac_b200_bfgsfit_channels.restype = C.c_int
+        L.dirac_b200_bfgsfit_channels.argtypes = [c_double_p] * 4 + [C.c_int] * 3 + [
+            C.POINTER(baseline_t), C.POINTER(clus_source_t), C.c_int, C.c_int, c_double_p, C.c_int,
+            C.c_double, C.c_double, C.c_double, c_double_p, C.c_int, C.c_int, C.c_int, C.c_double,
+            C.c_int, C.c_double, c_double_p, c_double_p, c_double_p]
+        freqs = np.ascontiguousarray(freqs, dtype=np.float64)
+        nchan = len(freqs)
+        r0, r1 = np.zeros(nchan), np.zeros(nchan)
+        pfreq = np.zeros((nchan, len(p))) if keep_pfreq else None
+        rv = L.dirac_b200_bfgsfit_channels(
+            dptr(u), dptr(v), dptr(w), dptr(xo), N, Nbase, tilesz, barr, sky.arr, sky.M, sky.Mt,
+            dptr(freqs), nchan, deltafch, uvmin, uvmax, dptr(p), max_lbfgs, lbfgs_m, solver_mode,
+            mean_nu, ccid, rho, dptr(r0), dptr(r1),
+            dptr(pfreq.reshape(-1)) if keep_pfreq else None)
+        return rv, r0, r1, pfreq
+
     def recalculate_diffuse_coherencies(self, u, v, w, x, N, barr, sky: SkyModel, freq0, fdelta, cid,
                                         sh_n0, sh_beta, Z, tdelta=10.0, dec0=1.0, uvmin=0.0,
                                         uvmax=1e9, Nt=4, use_cuda=0):

@@ -49,6 +49,9 @@ WITHSOL_EXPORTED = [
 #: every symbol include/dirac_b200_diffuse.h declares (diffuse cluster from a spatial model)
 DIFFUSE_EXPORTED = ["recalculate_diffuse_coherencies", "dirac_b200_diffuse_coherencies"]
 
+#: every symbol include/dirac_b200_channels.h declares (per-channel refinement, driver option -b 1)
+CHANNELS_EXPORTED = ["calculate_residuals", "dirac_b200_bfgsfit_channels", "dirac_b200_transfer_stats"]
+
 
 class DiracB200(DiracAPI):
     """The product library: the reference entry points (inherited bindings) plus the thin
@@ -107,6 +110,12 @@ class DiracB200(DiracAPI):
         self.lib.dirac_b200_comm_stats(C.byref(c), C.byref(b), C.byref(e), 1 if reset else 0)
         return dict(host_syncs=n.value, host_wait_s=w.value, collectives=c.value,
                     collective_bytes=b.value, collective_enqueue_s=e.value)
+
+    def transfer_stats(self, reset=False):
+        """(sky models uploaded, bytes of coherencies copied between host and device)"""
+        n, b = C.c_ulonglong(0), C.c_ulonglong(0)
+        self.lib.dirac_b200_transfer_stats(C.byref(n), C.byref(b), 1 if reset else 0)
+        return n.value, b.value
 
     def noise_decisions(self, reset=False) -> int:
         self.lib.dirac_b200_noise_decisions.restype = C.c_long
