@@ -79,25 +79,12 @@ void diffuse_plan(const clus_source_t &c, int N, int sh_n0, double sh_beta, cons
   }
 }
 
-template <class T> T *upload(const std::vector<T> &h, cudaStream_t st) {
-  T *d = nullptr;
-  DB_CHECK(cudaMalloc((void **)&d, sizeof(T) * (h.size() ? h.size() : 1)));
-  if (!h.empty()) DB_CHECK(cudaMemcpyAsync(d, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice, st));
-  return d;
-}
-
 // a.pairs / rows / u, v, w / coh / R set by the caller; runs the kernels and waits for them
-void diffuse_run(const DiffusePlan &pl, DiffuseArgs a, cudaStream_t st) {
-  DiffuseSource *dsrc = upload(pl.src, st);
-  double2 *dscoh = upload(pl.scoh, st), *dZt = upload(pl.Zt, st);
-  double *dcf = upload(pl.cf, st);
-  double2 *dcjq = nullptr;
-  DB_CHECK(cudaMalloc((void **)&dcjq, sizeof(double2) * pl.ncjq));
-  a.src = dsrc; a.ns = (int)pl.src.size(); a.Zt = dZt; a.scoh = dscoh; a.cf = dcf; a.cjq = dcjq;
-  db_launch_diffuse(&a, pl.max_n0, st);
-  db_stream_sync(st);
-  DB_CHECK(cudaGetLastError());
-  cudaFree(dsrc); cudaFree(dscoh); cudaFree(dZt); cudaFree(dcf); cudaFree(dcjq);
+void diffuse_run(DeviceScope &ds, const DiffusePlan &pl, DiffuseArgs a) {
+  a.src = ds.upload(pl.src); a.ns = (int)pl.src.size(); a.scoh = ds.upload(pl.scoh);
+  a.Zt = ds.upload(pl.Zt); a.cf = ds.upload(pl.cf); a.cjq = ds.alloc<double2>(pl.ncjq);
+  db_launch_diffuse(&a, pl.max_n0, ds.st);
+  ds.sync();
 }
 
 void check_cluster(int cid, int M) {
@@ -123,11 +110,7 @@ extern "C" int recalculate_diffuse_coherencies(double *u, double *v, double *w, 
   DiffusePlan pl;
   diffuse_plan(carr[cid], N, sh_n0, sh_beta, reinterpret_cast<const double2 *>(Z), &pl);
   if (pl.src.empty() || Nbase <= 0) return 0;  // no source: the slot is left as it is
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    fprintf(stderr, "dirac_b200: no CUDA device available. This library has no CPU fallback.\n");
-    exit(1);
-  }
+  DeviceScope ds;
   const long long R = Nbase;
   // rows grouped by station pair (counting sort); rows naming a station outside 0..N-1 share one
   // group that gets zeros
@@ -149,31 +132,21 @@ extern "C" int recalculate_diffuse_coherencies(double *u, double *v, double *w, 
     row_off.push_back(cnt[k]);
   }
   row_off.push_back(R);
-  cudaStream_t st;
-  DB_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   DiffuseArgs a;
   memset(&a, 0, sizeof(a));
   a.N = N; a.sh = sh_n0;
-  short2 *dpairs = upload(pairs, st);
-  long long *doff = upload(row_off, st), *drows = upload(rows, st);
-  a.pairs = dpairs; a.npairs = (int)pairs.size(); a.row_off = doff; a.rows = drows;
-  const std::vector<double> uvw[3] = {std::vector<double>(u, u + R), std::vector<double>(v, v + R),
-                                       std::vector<double>(w, w + R)};
-  a.u = upload(uvw[0], st);
-  a.v = upload(uvw[1], st);
-  a.w = upload(uvw[2], st);
+  a.pairs = ds.upload(pairs); a.npairs = (int)pairs.size();
+  a.row_off = ds.upload(row_off); a.rows = ds.upload(rows);
+  a.u = ds.upload(u, R); a.v = ds.upload(v, R); a.w = ds.upload(w, R);
   a.freq0 = freq0; a.fdelta2 = fdelta * 0.5; a.R = R;
-  DB_CHECK(cudaMalloc((void **)&a.coh, sizeof(double2) * 4 * R));
-  diffuse_run(pl, a, st);
+  a.coh = ds.alloc<double2>(4 * R);
+  diffuse_run(ds, pl, a);
   // only cluster cid's slice comes back: planar [4][R] -> x[row][cid][4]
   std::vector<double2> h((size_t)4 * R);
   DB_CHECK(cudaMemcpy(h.data(), a.coh, sizeof(double2) * 4 * R, cudaMemcpyDeviceToHost));
   double2 *X = reinterpret_cast<double2 *>(x);
   for (long long r = 0; r < R; r++)
     for (int c = 0; c < 4; c++) X[((size_t)r * M + cid) * 4 + c] = h[(size_t)c * R + r];
-  cudaFree(a.coh); cudaFree((void *)a.u); cudaFree((void *)a.v); cudaFree((void *)a.w);
-  cudaFree(dpairs); cudaFree(doff); cudaFree(drows);
-  cudaStreamDestroy(st);
   return 0;
 }
 
@@ -191,18 +164,11 @@ extern "C" int dirac_b200_diffuse_coherencies(dirac_b200_problem *pr, const doub
   memset(&a, 0, sizeof(a));
   a.N = d.N; a.sh = sh_n0;
   a.pairs = d.blpq; a.npairs = d.Nbase; a.ntime = d.tilesz; a.Nbase = d.Nbase;
-  double *du = nullptr, *dv = nullptr, *dw = nullptr;
-  DB_CHECK(cudaMalloc((void **)&du, sizeof(double) * 3 * d.R));
-  dv = du + d.R;
-  dw = dv + d.R;
-  DB_CHECK(cudaMemcpyAsync(du, u, sizeof(double) * d.R, cudaMemcpyHostToDevice, d.stream));
-  DB_CHECK(cudaMemcpyAsync(dv, v, sizeof(double) * d.R, cudaMemcpyHostToDevice, d.stream));
-  DB_CHECK(cudaMemcpyAsync(dw, w, sizeof(double) * d.R, cudaMemcpyHostToDevice, d.stream));
-  a.u = du; a.v = dv; a.w = dw;
+  DeviceScope ds(d.stream);
+  a.u = ds.upload(u, d.R); a.v = ds.upload(v, d.R); a.w = ds.upload(w, d.R);
   a.freq0 = freq0; a.fdelta2 = fdelta * 0.5; a.R = d.R;
   a.coh = d.coh + (size_t)cid * 4 * d.R;
-  diffuse_run(pl, a, d.stream);
-  cudaFree(du);
+  diffuse_run(ds, pl, a);
   // the Gram tensors cached for LM belong to the old coherencies (every solve also rebuilds them)
   if (pr->lm.ready) memset(pr->lm.T_valid, 0, d.Mt);
   return 0;

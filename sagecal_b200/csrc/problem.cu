@@ -107,7 +107,7 @@ int db_sm_count() {
   return n[dev];
 }
 
-static void require_gpu() {
+void require_gpu() {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess || n == 0) {
@@ -186,6 +186,24 @@ void db_free(void *p) {
     g_free_blocks.insert({bytes, p});
     g_cached_bytes += bytes;
   }
+}
+
+static cudaStream_t new_call_stream() {
+  require_gpu();
+  cudaStream_t st;
+  DB_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  return st;
+}
+DeviceScope::DeviceScope() : st(new_call_stream()), own_(true) {}
+DeviceScope::DeviceScope(cudaStream_t borrowed) : st(borrowed), own_(false) {}
+DeviceScope::~DeviceScope() {
+  cudaStreamSynchronize(st);
+  for (void *p : bufs_) cudaFree(p);
+  if (own_) cudaStreamDestroy(st);
+}
+void DeviceScope::sync() {
+  db_stream_sync(st);
+  DB_CHECK(cudaGetLastError());
 }
 
 template <typename T>
@@ -430,22 +448,25 @@ extern "C" void dirac_b200_set_data(dirac_b200_problem *pr, const double *x) {
   db_stream_sync(pr->d.stream);
 }
 
-extern "C" void dirac_b200_get_coherencies(dirac_b200_problem *pr, double *coh) {
-  DevProblem &d = pr->d;
-  long long rows_per = (128ll << 20) / ((long long)d.M * 64);
+void db_download_coh(const double2 *coh, double *x, int M, long long R, cudaStream_t st) {
+  long long rows_per = (128ll << 20) / ((long long)M * 64);
   if (rows_per < 1) rows_per = 1;
-  if (rows_per > d.R) rows_per = d.R;
-  double2 *stage = dev_alloc<double2>((size_t)rows_per * d.M * 4);
-  for (long long r0 = 0; r0 < d.R; r0 += rows_per) {
-    int nr = (int)((d.R - r0 < rows_per) ? (d.R - r0) : rows_per);
-    db_launch_coh_from_planar(d.coh, stage, r0, nr, d.M, d.R, d.stream);
+  if (rows_per > R) rows_per = R;
+  double2 *stage = dev_alloc<double2>((size_t)rows_per * M * 4);
+  for (long long r0 = 0; r0 < R; r0 += rows_per) {
+    int nr = (int)((R - r0 < rows_per) ? (R - r0) : rows_per);
+    db_launch_coh_from_planar(coh, stage, r0, nr, M, R, st);
     db_count_launch(1);
-    DB_CHECK(cudaMemcpyAsync(coh + (size_t)r0 * d.M * 8, stage, (size_t)nr * d.M * 64,
-                             cudaMemcpyDeviceToHost, d.stream));
+    DB_CHECK(cudaMemcpyAsync(x + (size_t)r0 * M * 8, stage, (size_t)nr * M * 64,
+                             cudaMemcpyDeviceToHost, st));
   }
-  db_stream_sync(d.stream);
-  db_count_coh_host_bytes((size_t)d.R * d.M * 64);
+  db_stream_sync(st);
+  db_count_coh_host_bytes((size_t)R * M * 64);
   db_free(stage);
+}
+
+extern "C" void dirac_b200_get_coherencies(dirac_b200_problem *pr, double *coh) {
+  db_download_coh(pr->d.coh, coh, pr->d.M, pr->d.R, pr->d.stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -3,6 +3,8 @@
 #include <cusolverDn.h>
 #include <cublas_v2.h>
 
+#include <vector>
+
 #include "internal.cuh"
 
 struct LMWork {
@@ -89,6 +91,46 @@ void db_flag_wait(const volatile unsigned long long *flag, unsigned long long ep
                   cudaStream_t st);
 void *db_malloc(size_t bytes);
 void db_free(void *p);
+// exits with a message if there is no CUDA device: this library has no CPU fallback
+void require_gpu();
+
+// Device state of one call: a non-blocking stream, created here (after require_gpu) or borrowed from a
+// resident problem, and the cudaMalloc buffers allocated through alloc / upload.  The destructor waits
+// for the stream (uncounted: on the normal path the call has already synced), frees the buffers and
+// destroys the stream if it created it.
+class DeviceScope {
+ public:
+  DeviceScope();
+  explicit DeviceScope(cudaStream_t borrowed);
+  ~DeviceScope();
+  DeviceScope(const DeviceScope &) = delete;
+  DeviceScope &operator=(const DeviceScope &) = delete;
+  template <class T> T *alloc(size_t n) {
+    void *p = nullptr;
+    DB_CHECK(cudaMalloc(&p, sizeof(T) * n));
+    bufs_.push_back(p);
+    return (T *)p;
+  }
+  // at least one element is allocated, so that an empty table is still a valid pointer; the host
+  // array must stay alive until the next wait on st
+  template <class T> T *upload(const T *h, size_t n) {
+    T *d = alloc<T>(n ? n : 1);
+    if (n) DB_CHECK(cudaMemcpyAsync(d, h, sizeof(T) * n, cudaMemcpyHostToDevice, st));
+    return d;
+  }
+  template <class T> T *upload(const std::vector<T> &h) { return upload(h.data(), h.size()); }
+  // the counted host wait (dirac_b200_host_stats), then the check for a failed launch
+  void sync();
+  const cudaStream_t st;
+
+ private:
+  const bool own_;
+  std::vector<void *> bufs_;
+};
+
+// planar [M][4][R] device coherencies -> host x[row][M][8] (the API layout) through a db_malloc stage
+// of at most 128 MB; waits for the copies once and counts the bytes (dirac_b200_transfer_stats)
+void db_download_coh(const double2 *coh, double *x, int M, long long R, cudaStream_t st);
 void db_count_launch(int n);
 void db_prof_begin(int kind, double bytes, cudaStream_t st);
 void db_prof_end(cudaStream_t st);
