@@ -492,7 +492,8 @@ unsigned long long dirac_b200_launch_count(void);
  * kind: 0 full predict, 1 LBFGS gradient, 2 k_cluster_pass*, 3 k_coh_gram, 4 assembly, 5 damped solve
  * (k_chol_solve / k_tri_solve / batched potrf), 6 k_weighted_jtj, 7 line setup, 8 k_cluster_pass
  * without gradient (ADD / SUB / cost-only; kind 2 then counts the gradient-carrying INIT / TRIAL passes),
- * 9 k_rtr_stats (row condensation of the RTR / NSD solvers), 10 k_rtr_eval.  enable(1) clears the
+ * 9 k_rtr_stats (row condensation of the RTR / NSD solvers), 10 k_rtr_eval, 13 k_stream_band (cost
+ * or residual of every channel of a minibatch band), 14 k_grad_tma_band (its gradient).  enable(1) clears the
  * records; read returns the launch count and sums the elapsed
  * milliseconds and the algorithmic bytes of the recorded launches of that kind. */
 unsigned long long dirac_b200_kernel_count(int kind); /* launches of `kind` since load */
@@ -531,4 +532,6 @@ int dirac_b200_bigtri_solve(int n, const double *L, const double *b, double *x, 
 #include "dirac_b200_diffuse.h"
 /* per-channel refinement (calculate_residuals and the channel loop on one resident problem) */
 #include "dirac_b200_channels.h"
+/* stochastic calibration of a whole solution interval (the minibatch driver's loop in one call) */
+#include "dirac_b200_stochastic.h"
 #endif

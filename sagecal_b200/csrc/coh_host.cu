@@ -6,6 +6,7 @@
 
 #include "../../include/dirac_b200.h"
 #include "../../include/dirac_b200_channels.h"
+#include "../../include/dirac_b200_stochastic.h"
 #include "coh.h"
 #include "problem.h"
 
@@ -710,6 +711,111 @@ extern "C" int dirac_b200_bfgsfit_channels(double *u, double *v, double *w, doub
     db_free(dx);
   }
   dirac_b200_destroy(pr);
+  return 0;
+}
+// The stochastic calibration of one interval (minibatch_mode.cpp:368-506, no beam) in one call.  Device
+// storage for the whole interval: the coherencies coh[minibatch][chan][M][4][R] (planar, so that a band
+// of a minibatch is one contiguous [nc][M][4][R] block), the data twice, [minibatch][chan][R][4] for
+// the residual kernel and planar [minibatch][chan][4][R] for the fits, and two sets of flags: as
+// preset (every later epoch re-presets the flags on each load) and with the first epoch's uv cut.
+extern "C" int dirac_b200_stochastic_interval(double *u, double *v, double *w, double *xo, int N,
+                                              int Nbase, int tmb, int minibatches, baseline_t *barr,
+                                              clus_source_t *carr, int M, int Mt, double *freqs,
+                                              int Nchan, double deltaf, double uvmin, double uvmax,
+                                              int nsolbw, int nepochs, int max_lbfgs, int lbfgs_m,
+                                              double robust_nu, persistent_data_t *pt,
+                                              double *pfreq, int ccid, double rho, int phase_only,
+                                              double *res_00, double *res_01) {
+  if (nsolbw < 1 || nsolbw > Nchan) {
+    fprintf(stderr, "dirac_b200_stochastic_interval: nsolbw = %d bands of Nchan = %d channels; the "
+                    "driver clamps nsolbw to Nchan, this call takes 1 <= nsolbw <= Nchan\n",
+            nsolbw, Nchan);
+    return -1;
+  }
+  const long long R = (long long)Nbase * tmb;
+  const size_t m = (size_t)8 * N * Mt;
+  // bands (minibatch_mode.cpp:93-116): ceil(Nchan / nsolbw) channels each, the last one the rest
+  const int nper = (Nchan + nsolbw - 1) / nsolbw;
+  std::vector<int> c0(nsolbw), nc(nsolbw);
+  for (int b = 0, count = 0; b < nsolbw; b++) {
+    nc[b] = count + nper < Nchan ? nper : Nchan - count;
+    c0[b] = count;
+    count += nc[b];
+  }
+  std::vector<unsigned char> hflag((size_t)minibatches * R);
+  for (int mb = 0; mb < minibatches; mb++)
+    db_canonical_flags(N, Nbase, tmb, barr + (size_t)mb * R, hflag.data() + (size_t)mb * R);
+  DeviceScope ds;
+  CohArgs a = stage_sky(ds, carr, M, u, v, w, (long long)minibatches * R, freqs, Nchan,
+                        deltaf / (double)Nchan);
+  const double *du = a.u, *dv = a.v, *dw = a.w, *df = a.freqs;
+  a.R = R; a.N = N;
+  unsigned char *flag_preset = ds.upload(hflag);
+  unsigned char *flag_cut = ds.upload(hflag);
+  const size_t nvis = (size_t)minibatches * Nchan * R * 4;
+  double2 *xapi = ds.upload((const double2 *)xo, nvis);
+  double2 *xpl = ds.alloc<double2>(nvis);
+  double2 *coh = (double2 *)db_malloc(sizeof(double2) * (size_t)M * nvis);
+  for (int mb = 0; mb < minibatches; mb++) {
+    a.u = du + (size_t)mb * R; a.v = dv + (size_t)mb * R; a.w = dw + (size_t)mb * R;
+    a.flag = flag_cut + (size_t)mb * R;
+    for (int c = 0; c < Nchan; c++) {
+      const size_t mc = (size_t)mb * Nchan + c;
+      db_launch_vis_to_planar(xapi + mc * 4 * R, xpl + mc * 4 * R, R, ds.st);
+      // the uv cut of precalculate_coherencies_multifreq (predict.c:731-735)
+      a.freqs = df + c;
+      a.Nchan = 1;
+      a.uvmin = c == 0 ? uvmin : 0.0;
+      a.uvmax = c == Nchan - 1 ? uvmax : 1e300;
+      a.coh = coh + mc * M * 4 * R;
+      db_launch_coherencies(&a, ds.st);
+      db_count_launch(2);
+    }
+  }
+  // epochs x minibatches x bands of the minibatch LBFGS; the uv cut holds in the first epoch only
+  BandDev *bd = db_band_create(N, Nbase, tmb, carr, M, Mt, nper, ds.st);
+  for (int ep = 0; ep < nepochs; ep++)
+    for (int mb = 0; mb < minibatches; mb++)
+      for (int b = 0; b < nsolbw; b++) {
+        const size_t mc = (size_t)mb * Nchan + c0[b];
+        const BandView bv = {coh + mc * M * 4 * R, xpl + mc * 4 * R,
+                             (ep == 0 ? flag_cut : flag_preset) + (size_t)mb * R, nc[b]};
+        const size_t o = ((size_t)ep * minibatches + mb) * nsolbw + b;
+        db_band_fit(bd, bv, pfreq + b * m, nullptr, nullptr, nullptr, max_lbfgs, lbfgs_m, robust_nu,
+                    res_00 + o, res_01 + o, pt + b);
+      }
+  db_band_destroy(bd);
+  // residuals of every minibatch and band with the band's solution (calculate_residuals_multifreq)
+  a.coh = nullptr; a.flag = nullptr;
+  const ResidualTables tb = residual_tables(ds, barr, carr, N, M, residual_coef(carr, M), ccid, &a);
+  const int cm = tb.cm;
+  a.pinv_nchunk = cm >= 0 ? carr[cm].nchunk : 1;
+  double *dp = ds.alloc<double>(tb.npar > 0 ? (size_t)tb.npar : 1);
+  double *dpinv = cm >= 0 ? ds.alloc<double>((size_t)8 * N * carr[cm].nchunk) : nullptr;
+  std::vector<double> pinv;
+  for (int b = 0; b < nsolbw; b++) {
+    if (nc[b] == 0) continue;
+    DB_CHECK(cudaMemcpyAsync(dp, pfreq + b * m, sizeof(double) * tb.npar, cudaMemcpyHostToDevice,
+                             ds.st));
+    if (cm >= 0) {
+      correction_inverse(pfreq + b * m, carr[cm], N, rho, phase_only, pinv);
+      DB_CHECK(cudaMemcpyAsync(dpinv, pinv.data(), sizeof(double) * pinv.size(),
+                               cudaMemcpyHostToDevice, ds.st));
+    }
+    a.p = dp; a.pinv = dpinv; a.freqs = df + c0[b]; a.Nchan = nc[b];
+    for (int mb = 0; mb < minibatches; mb++) {
+      a.u = du + (size_t)mb * R; a.v = dv + (size_t)mb * R; a.w = dw + (size_t)mb * R;
+      a.xout = xapi + ((size_t)mb * Nchan + c0[b]) * 4 * R;
+      db_prof_begin(11, 128.0 * (double)R * nc[b], ds.st);
+      db_launch_residual_multifreq(&a, ds.st);
+      db_prof_end(ds.st);
+      db_count_launch(1);
+    }
+    db_stream_sync(ds.st);  // dp and dpinv are rewritten by the next band
+  }
+  DB_CHECK(cudaMemcpyAsync(xo, xapi, sizeof(double2) * nvis, cudaMemcpyDeviceToHost, ds.st));
+  ds.sync();
+  db_free(coh);
   return 0;
 }
 // Dirac_radio.h:666 (residual.c:1620-1740): simulation with solutions

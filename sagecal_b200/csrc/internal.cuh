@@ -366,6 +366,8 @@ void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st);
 // the gradient of rows [r_lo, r_hi) only: the time blocks that overlap them
 void db_launch_grad_window_tma(const GradArgs *a, int ntile, long long r_lo, long long r_hi,
                                cudaStream_t st);
+// every channel of a band: a holds the first channel's coh / res, the grid's z axis the channels
+void db_launch_grad_band_tma(const GradArgs *a, int ntile, int nchan, cudaStream_t st);
 int db_cluster_pass_nblocks(int ntile, int nt, int tslice);
 void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st);
 // whether plain (unweighted) passes of this array take k_cluster_pass_lin, the one variant that
@@ -394,6 +396,12 @@ void db_launch_bigtri_solve(const double *L, int ld, int n, const double *b, dou
 int db_stream_all_nblocks(int Nbase, int tilesz);
 void db_launch_predict_tma(const StreamAllArgs *a, cudaStream_t st);
 void db_launch_cost_window_tma(const StreamAllArgs *a, cudaStream_t st);
+// kernels_band.cu: MODE 0 of k_stream_all over the nchan channels of a band in one launch; a holds the
+// first channel's coh / x / out, the others follow at strides M 4 R and 4 R.  The cost's partials
+// need db_band_nblocks entries.
+int db_band_nblocks(int Nbase, int tilesz, int nchan);
+void db_launch_band_tma(const StreamAllArgs *a, int nchan, cudaStream_t st);
+void db_launch_band_tma(const StreamAllArgs *a, int nchan, cudaStream_t st);
 void db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st);
 // (TB, NST, WARPS) of the last k_stream_all<1> launch since the reset (-1 each: none)
 void db_line_setup_shape_reset();

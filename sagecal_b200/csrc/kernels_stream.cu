@@ -3,6 +3,7 @@
 // 32 consecutive stations q, 512 contiguous bytes per polarisation product per timeslot).
 //
 //   k_grad_tma_split : LBFGS gradient over all clusters from a stored residual
+//   k_grad_tma_band  : the same over every channel of a band into one gradient (minibatch LBFGS)
 //                      (replaces cpu_calc_deriv(_robust), robust_lbfgs.c:424-560,155-316, which
 //                       loop per PARAMETER over all rows; here one pass over rows)
 //   k_cluster_pass*  : per-cluster E-step pass of the LM solver: model of one cluster, residual,
@@ -154,8 +155,14 @@ __device__ __forceinline__ double warp_reduce4(double v0, double v1, double v2, 
 // robust_batchmode_lbfgs.c:347-500): the grid's time blocks start at a.tb0, and rows outside the
 // window count like flagged rows (their residual is not read).
 // ------------------------------------------------------------------------------------------------
-template <int TB, int NST, bool WIN>
+// BAND: one channel of a band per blockIdx.z ([chan][M][4][R] coherencies, [chan][4][R] residual), all
+// channels accumulating into the one gradient
+template <int TB, int NST, bool WIN, bool BAND = false>
 __device__ __forceinline__ void grad_tma_split_body(GradArgs a) {
+  if (BAND) {
+    a.coh += (long long)blockIdx.z * a.M * 4 * a.R;
+    a.res += (long long)blockIdx.z * 4 * a.R;
+  }
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int STAGE_ELEMS = TB * 4 * 32;  // double2 per stage
   double (*sq)[8][TILE_Q] = reinterpret_cast<double (*)[8][TILE_Q]>(smem_raw);
@@ -334,6 +341,12 @@ template <int TB, int NST>
 __global__ void __launch_bounds__(2 * TILE_THREADS)
 k_grad_tma_window(GradArgs a) {
   grad_tma_split_body<TB, NST, true>(a);
+}
+
+template <int TB, int NST>
+__global__ void __launch_bounds__(2 * TILE_THREADS)
+k_grad_tma_band(GradArgs a) {
+  grad_tma_split_body<TB, NST, false, true>(a);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -900,6 +913,20 @@ void db_launch_grad_tma(const GradArgs *a, int ntile, cudaStream_t st) {
   }
   dim3 grid(ntile, (a->tilesz + TB - 1) / TB);
   k_grad_tma_split<TB, NST><<<grid, 2 * TILE_THREADS, smem, st>>>(*a);
+}
+
+void db_launch_grad_band_tma(const GradArgs *a, int ntile, int nchan, cudaStream_t st) {
+  constexpr int TB = 4, NST = 2;
+  const size_t smem = sizeof(double) * 2 * TILE_P * 8 * TILE_Q +
+                      (size_t)TILE_P * NST * TB * 4 * 32 * sizeof(double2) + TILE_P * NST * 8;
+  static bool configured = false;
+  if (!configured) {
+    DB_CHECK(cudaFuncSetAttribute(k_grad_tma_band<TB, NST>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured = true;
+  }
+  dim3 grid(ntile, (a->tilesz + TB - 1) / TB, nchan);
+  k_grad_tma_band<TB, NST><<<grid, 2 * TILE_THREADS, smem, st>>>(*a);
 }
 
 void db_launch_grad_window_tma(const GradArgs *a, int ntile, long long r_lo, long long r_hi,

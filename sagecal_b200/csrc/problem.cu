@@ -34,12 +34,13 @@ static cudaEvent_t prof_event() {
   DB_CHECK(cudaEventCreate(&e));
   return e;
 }
-static unsigned long long g_kind_count[13] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+// kinds: 13 k_stream_band (band cost or residual), 14 k_grad_tma_band (band gradient)
+static unsigned long long g_kind_count[15] = {0};
 extern "C" unsigned long long dirac_b200_kernel_count(int kind) {
-  return (kind >= 0 && kind < 13) ? g_kind_count[kind] : 0ull;
+  return (kind >= 0 && kind < 15) ? g_kind_count[kind] : 0ull;
 }
 void db_prof_begin(int kind, double bytes, cudaStream_t st) {
-  if (kind >= 0 && kind < 13) g_kind_count[kind]++;
+  if (kind >= 0 && kind < 15) g_kind_count[kind]++;
   if (!g_prof_on) return;
   ProfRec r; r.a = prof_event(); r.b = prof_event(); r.kind = kind; r.bytes = bytes;
   DB_CHECK(cudaEventRecord(r.a, st));
@@ -211,7 +212,7 @@ static T *dev_alloc(size_t n) {
   return (T *)db_malloc(n * sizeof(T) + 16);
 }
 
-static void build_tiles(int N, std::vector<TileDesc> &tiles) {
+void db_build_tiles(int N, std::vector<TileDesc> &tiles) {
   int npb = (N - 1 + TILE_P - 1) / TILE_P;  // p in [0, N-2]
   int nqb = (N + TILE_Q - 1) / TILE_Q;
   for (int pb = 0; pb < npb; pb++)
@@ -263,6 +264,43 @@ extern "C" void dirac_b200_set_comm(dirac_b200_problem *pr, int rank, int world,
 }
 
 
+// the row order must be the canonical one (baseline_utils.c:445-461): checked, bit-exact
+// (15.7 M rows at 512 stations x 120 timeslots: shared out over a few host threads by timeslot)
+void db_canonical_flags(int N, int Nbase, int tilesz, const baseline_t *barr, unsigned char *hflag) {
+  const long long R = (long long)Nbase * tilesz;
+  const long long Nb = (long long)N * (N - 1) / 2;
+  int nthr = (R > (1 << 20)) ? 8 : 1;
+  if (nthr > tilesz) nthr = tilesz;
+  std::vector<long long> bad(nthr, -1);
+  auto work = [&](int th) {
+    for (int t = th; t < tilesz; t += nthr) {
+      long long r = (long long)t * Nb;
+      for (int p = 0; p < N - 1; p++)
+        for (int q = p + 1; q < N; q++, r++) {
+          if (barr[r].sta1 != p || barr[r].sta2 != q) {
+            if (bad[th] < 0) bad[th] = r;
+            return;
+          }
+          hflag[r] = barr[r].flag;
+        }
+    }
+  };
+  if (nthr == 1) {
+    work(0);
+  } else {
+    std::vector<std::thread> pool;
+    for (int th = 0; th < nthr; th++) pool.emplace_back(work, th);
+    for (auto &th : pool) th.join();
+  }
+  for (int th = 0; th < nthr; th++)
+    if (bad[th] >= 0) {
+      const long long r = bad[th];
+      fprintf(stderr, "dirac_b200: barr[%lld]=(%d,%d) is not in the canonical order of "
+                      "generate_baselines; unsupported row order\n", r, barr[r].sta1, barr[r].sta2);
+      exit(1);
+    }
+}
+
 static dirac_b200_problem *create_impl(int N, int Nbase, int tilesz, const baseline_t *barr,
                                        const clus_source_t *carr, int M, int Mt, const double *coh,
                                        const double *x, long long npar) {
@@ -293,42 +331,9 @@ static dirac_b200_problem *create_impl(int N, int Nbase, int tilesz, const basel
   pr->vis_stage = dev_alloc<double2>((size_t)4 * R);
   if (x) db_upload_vis(pr, x, d.x);
 
-  // --- row order must be the canonical one (baseline_utils.c:445-461): checked, bit-exact ---
-  // (15.7 M rows at 512 stations x 120 timeslots: shared out over a few host threads by timeslot)
+  // --- row order must be the canonical one ---
   std::vector<unsigned char> hflag(R);
-  {
-    const long long Nb = (long long)N * (N - 1) / 2;
-    int nthr = (R > (1 << 20)) ? 8 : 1;
-    if (nthr > tilesz) nthr = tilesz;
-    std::vector<long long> bad(nthr, -1);
-    auto work = [&](int th) {
-      for (int t = th; t < tilesz; t += nthr) {
-        long long r = (long long)t * Nb;
-        for (int p = 0; p < N - 1; p++)
-          for (int q = p + 1; q < N; q++, r++) {
-            if (barr[r].sta1 != p || barr[r].sta2 != q) {
-              if (bad[th] < 0) bad[th] = r;
-              return;
-            }
-            hflag[r] = barr[r].flag;
-          }
-      }
-    };
-    if (nthr == 1) {
-      work(0);
-    } else {
-      std::vector<std::thread> pool;
-      for (int th = 0; th < nthr; th++) pool.emplace_back(work, th);
-      for (auto &th : pool) th.join();
-    }
-    for (int th = 0; th < nthr; th++)
-      if (bad[th] >= 0) {
-        const long long r = bad[th];
-        fprintf(stderr, "dirac_b200: barr[%lld]=(%d,%d) is not in the canonical order of "
-                        "generate_baselines; unsupported row order\n", r, barr[r].sta1, barr[r].sta2);
-        exit(1);
-      }
-  }
+  db_canonical_flags(N, Nbase, tilesz, barr, hflag.data());
   d.flag = dev_alloc<unsigned char>(R);
   DB_CHECK(cudaMemcpyAsync(d.flag, hflag.data(), R, cudaMemcpyHostToDevice, d.stream));
   db_stream_sync(d.stream);  // data and flags are up (hflag goes out of scope)
@@ -355,7 +360,7 @@ static dirac_b200_problem *create_impl(int N, int Nbase, int tilesz, const basel
 
   // --- tiles ---
   std::vector<TileDesc> tiles;
-  build_tiles(N, tiles);
+  db_build_tiles(N, tiles);
   d.ntile = (int)tiles.size();
   d.tiles = dev_alloc<TileDesc>(tiles.size());
   DB_CHECK(cudaMemcpy(d.tiles, tiles.data(), sizeof(TileDesc) * tiles.size(),

@@ -5,6 +5,7 @@
 
 #include <vector>
 
+#include "../../include/dirac_b200.h"
 #include "internal.cuh"
 
 struct LMWork {
@@ -176,6 +177,41 @@ void db_launch_cluster_rowmap(const double2 *coh_k, const double2 *in, const dou
                               const int *chunk_poff, int nchunk, const short2 *blpq, long long R,
                               int Nbase, int sign, double beta, cudaStream_t st);
 }
+
+// ---- minibatch bands (minibatch.cu) ---------------------------------------------------------------
+// A band: channels [c0, c0 + nc) of one minibatch, coherencies [nc][M][4][R] and data [nc][4][R] in the
+// planar layout, the flags of the minibatch's R rows.  BandDev is the device state the bands of one
+// shape share: chunk tables, tiles, station pairs, the Jones, the gradient, the residual of up to maxnc
+// channels and the scratch of the one-launch cost reduction.
+struct BandView {
+  const double2 *coh, *x;
+  const unsigned char *flag;
+  int nc;
+};
+struct BandDev {
+  int N, Nbase, tilesz, M, Mt, maxnc, ntile;
+  long long R, npar;
+  ClusterDesc *clus;
+  int *chunk_poff;
+  TileDesc *tiles;
+  short2 *blpq;
+  double *pp, *g, *partials, *scal, *h_scal;
+  unsigned int *counters;
+  double2 *res;
+  cudaStream_t st;
+};
+void db_build_tiles(int N, std::vector<TileDesc> &tiles);
+// the flags of barr's R rows, after checking that they are in the canonical order of generate_baselines
+// (message and exit(1) otherwise, as dirac_b200_create)
+void db_canonical_flags(int N, int Nbase, int tilesz, const baseline_t *barr, unsigned char *flag);
+BandDev *db_band_create(int N, int Nbase, int tilesz, const clus_source_t *carr, int M, int Mt,
+                        int maxnc, cudaStream_t st);
+void db_band_destroy(BandDev *bd);
+// bfgsfit_minibatch_visibilities / _consensus on a resident band: res_0, res_1 the costs before and
+// after the fit over 8 R nc; p (host, 8 N Mt) in/out; y, z, rho: consensus terms or null
+void db_band_fit(BandDev *bd, const BandView &b, double *p, const double *y, const double *z,
+                 const double *rho, int max_lbfgs, int lbfgs_m, double robust_nu, double *res_0,
+                 double *res_1, persistent_data_t *indata);
 
 void db_lm_free(dirac_b200_problem *pr);
 void db_rtr_free(dirac_b200_problem *pr);

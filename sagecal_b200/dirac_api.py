@@ -56,6 +56,12 @@ class clus_source_t(C.Structure):
     ]
 
 
+class persistent_data_t(C.Structure):
+    """include/dirac_b200.h: the prefix of the reference's struct this library uses"""
+    _fields_ = [("y", C.c_void_p), ("s", C.c_void_p), ("rho", C.c_void_p), ("nfilled", C.c_int),
+                ("vacant", C.c_int), ("lbfgs_m", C.c_int), ("m", C.c_int), ("Nt", C.c_int)]
+
+
 class exinfo_gaussian(C.Structure):
     """Dirac_radio.h exinfo_gaussian — extended (Gaussian) source shape."""
     _fields_ = [("eX", C.c_double), ("eY", C.c_double), ("eP", C.c_double),
@@ -491,6 +497,40 @@ class DiracAPI:
         else:
             self.lib.bfgsfit_minibatch_consensus(*head, dptr(Y), dptr(Z), dptr(rho), *tail)
         return r0.value, r1.value
+
+    def stochastic_interval(self, u, v, w, xo, N, Nbase, tmb, barr, sky: SkyModel, freqs, deltaf, pt,
+                            pfreq, nsolbw, nepochs, uvmin=0.0, uvmax=1e9, max_lbfgs=4, lbfgs_m=5,
+                            robust_nu=2.0, ccid=-99999, rho=1e-9, phase_only=0):
+        """dirac_b200_stochastic_interval: the minibatch driver's loop over one interval in one call.
+        u, v, w [minibatches, Nbase*tmb]; xo [minibatches, Nchan, Nbase*tmb*8] data -> residual (in
+        place); barr: minibatches * Nbase*tmb rows (input only); pt: nsolbw persistent_data_t
+        (persist_init_array); pfreq [nsolbw, 8 N Mt] start -> solutions (in
+        place).  returns (retval, res_00, res_01), each [nepochs, minibatches, nsolbw]"""
+        L = self.lib
+        L.dirac_b200_stochastic_interval.restype = C.c_int
+        L.dirac_b200_stochastic_interval.argtypes = [c_double_p] * 4 + [C.c_int] * 4 + [
+            C.POINTER(baseline_t), C.POINTER(clus_source_t), C.c_int, C.c_int, c_double_p, C.c_int,
+            C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double,
+            C.c_void_p, c_double_p, C.c_int, C.c_double, C.c_int, c_double_p, c_double_p]
+        for a in (u, v, w, xo, pfreq):
+            assert a.dtype == np.float64 and a.flags.c_contiguous
+        freqs = np.ascontiguousarray(freqs, dtype=np.float64)
+        nmb = u.shape[0]
+        r0 = np.zeros((nepochs, nmb, nsolbw))
+        r1 = np.zeros((nepochs, nmb, nsolbw))
+        rv = L.dirac_b200_stochastic_interval(
+            dptr(u), dptr(v), dptr(w), dptr(xo), N, Nbase, tmb, nmb, barr, sky.arr, sky.M, sky.Mt,
+            dptr(freqs), len(freqs), deltaf, uvmin, uvmax, nsolbw, nepochs, max_lbfgs, lbfgs_m,
+            robust_nu, C.cast(pt, C.c_void_p), dptr(pfreq), ccid, rho, phase_only, dptr(r0), dptr(r1))
+        return rv, r0, r1
+
+    def persist_init_array(self, nbands, nminibatch, m, n, lbfgs_m, Nt=4):
+        """nbands persistent_data_t of include/dirac_b200.h back to back, as the driver's
+        ptdata_array, each initialised by lbfgs_persist_init"""
+        arr = (persistent_data_t * nbands)()
+        for b in range(nbands):
+            self.lib.lbfgs_persist_init(C.byref(arr[b]), nminibatch, m, n, lbfgs_m, Nt)
+        return arr
 
     def sagefit_visibilities_admm(self, u, v, w, x, N, Nbase, tilesz, barr, sky, coh, pp, Y, BZ, rho,
                                   max_emiter=3, max_iter=2, nulow=2.0, nuhigh=30.0, Nt=4,
