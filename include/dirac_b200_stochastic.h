@@ -2,7 +2,8 @@
  * dirac_b200 — stochastic calibration of a whole solution interval (`sagecal -N <epochs>
  * -M <minibatches> -w <bands>`, src/MS/minibatch_mode.cpp:364-509, without beams): the driver's loop
  * over epochs, minibatches and bands of channels in one call, with every coherency predicted straight
- * into device memory and kept there for the whole interval.
+ * into device memory and kept there for the whole interval; and the same loop with spectral consensus
+ * over the bands (`-A <nadmm>`, src/MS/minibatch_consensus_mode.cpp:450-672).
  * include/dirac_b200.h includes this header; it may also be included on its own.
  */
 #ifndef DIRAC_B200_STOCHASTIC_H
@@ -56,6 +57,55 @@ int dirac_b200_stochastic_interval(double *u, double *v, double *w, double *xo, 
                                    int lbfgs_m, double robust_nu, persistent_data_t *pt, double *pfreq,
                                    int ccid, double rho, int phase_only, double *res_00,
                                    double *res_01);
+
+/* replaces minibatch_consensus_mode.cpp:453-672 for one interval when no beam is used (`sagecal -N
+ * <epochs> -M <minibatches> -w <bands> -A <nadmm>`, which main.cpp runs when nadmm > 1 and nsolbw > 1):
+ * the loop of dirac_b200_stochastic_interval inside nadmm ADMM iterations that tie the bands' Jones to
+ * a polynomial in frequency.  Per minibatch, every band b is fitted as bfgsfit_minibatch_consensus
+ * fits it, with y = Y_b, z = B_b Z and rho = rhok_b, and then dirac_b200_consensus_bands_update takes
+ * the ADMM step.  Y is the call's own and starts from zero.  The coherencies are predicted once, in
+ * (admm 0, epoch 0), and only that pass uses the uv cut.  robust_nu is fixed for the whole interval.
+ * The arguments up to phase_only are those of dirac_b200_stochastic_interval; then:
+ *   nadmm        ADMM iterations, >= 1
+ *   Npoly        polynomial terms, >= 1
+ *   B            [nsolbw][Npoly] the basis at the bands' mean frequencies (dirac_b200_consensus_basis)
+ *   Bi           [Mt][Npoly][Npoly] (dirac_b200_consensus_prod_inverse of B and rhok)
+ *   rhok         [nsolbw][Mt] the ADMM weight of every band and chunk
+ *   Z            [Mt][Npoly][8N] in/out: the global polynomial solution; the driver keeps it from one
+ *                interval to the next
+ *   use_global   != 0: every band's solution becomes B_b Z after the loop, and the residuals use it
+ *   res_00, res_01   [nadmm][nepochs][minibatches][nsolbw] out: every fit's cost before and after
+ *   res_0, res_1 out: the driver's running averages after the loop (see dirac_b200_consensus_bands_update)
+ *   fband        [nsolbw] out: the bad-band flags of the last minibatch
+ * What the driver does between intervals (resetting flagged bands and all bands,
+ * minibatch_consensus_mode.cpp:696-721) stays with the caller, which needs res_1 and fband for it.
+ * Returns 0, or -1 with a message on stderr and no output touched when nsolbw is outside [1, Nchan],
+ * nadmm < 1 or Npoly < 1. */
+int dirac_b200_stochastic_consensus_interval(
+    double *u, double *v, double *w, double *xo, int N, int Nbase, int tmb, int minibatches,
+    baseline_t *barr, clus_source_t *carr, int M, int Mt, double *freqs, int Nchan, double deltaf,
+    double uvmin, double uvmax, int nsolbw, int nepochs, int max_lbfgs, int lbfgs_m, double robust_nu,
+    persistent_data_t *pt, double *pfreq, int ccid, double rho, int phase_only, int nadmm, int Npoly,
+    double *B, double *Bi, double *rhok, double *Z, int use_global, double *res_00, double *res_01,
+    double *res_0, double *res_1, int *fband);
+
+/* the ADMM step of one minibatch of the consensus loop (minibatch_consensus_mode.cpp:540-601), host
+ * arithmetic, no device needed; for a host that keeps its own loop of bfgsfit_minibatch_consensus
+ * calls.  Decision for decision as the driver:
+ *   res_0 = (res_0 + sum_b res_00[b]) / nsolbw, res_1 likewise: a running mixture, not a mean;
+ *   fband[b] = 1 when resband[b] > 1.5 res_1, resband[b] = res_01[b] if res_00[b] > 0 and
+ *   res_01[b] > 0, else 1e12 (a NaN res_1 flags no band);
+ *   good bands: Y_b += rhok_b J_b;  z[p] = sum_b B_b[p] Y_b over band 0 whatever fband[0] says and the
+ *   good bands from 1 on;  Z = update_global_z_multi(z, Bi);  good bands: Y_b -= rhok_b B_b Z.
+ *   res_00, res_01   [nsolbw] the costs of this minibatch's fits
+ *   pfreq        [nsolbw][8 N Mt] the bands' Jones J_b
+ *   B, Bi, rhok  as dirac_b200_stochastic_consensus_interval takes them
+ *   res_0, res_1 in/out;  Y [nsolbw][8 N Mt] in/out;  Z [Mt][Npoly][8N] in/out;  fband [nsolbw] out
+ * Returns 0, or -1 with a message on stderr and nothing touched when N, Mt, nsolbw or Npoly is < 1. */
+int dirac_b200_consensus_bands_update(int N, int Mt, int nsolbw, int Npoly, const double *res_00,
+                                      const double *res_01, const double *pfreq, const double *B,
+                                      const double *Bi, const double *rhok, double *res_0,
+                                      double *res_1, double *Y, double *Z, int *fband);
 
 #ifdef __cplusplus
 }

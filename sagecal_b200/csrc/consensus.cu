@@ -12,6 +12,7 @@
 // setup_polynomials (consensus_poly.c:38-190) and find_prod_inverse_full (:380-545) and are pinned
 // against the compiled reference by the CPU tests.
 #include <math.h>
+#include <stdio.h>
 #include <string.h>
 #include <vector>
 
@@ -147,6 +148,97 @@ extern "C" int dirac_b200_consensus_prod_inverse(const double *B, double *Bi, in
           if (w[e] > 1e-12) s += V[i * n + e] * V[j * n + e] / w[e];
         out[i * n + j] = s;
       }
+  }
+  return 0;
+}
+
+// ---- the ADMM step of the spectral consensus over bands (minibatch_consensus_mode.cpp:524-601) ------
+// z = B_b Z of every chunk, as the driver sums it (:526-531): z[ci] = sum_p Bb[p] Z[ci][p]
+void db_consensus_bz(const double *Z, const double *Bb, int N, int Mt, int Npoly, double *z) {
+  const size_t n8 = (size_t)8 * N;
+  for (int ci = 0; ci < Mt; ci++) {
+    double *zc = z + n8 * ci;
+    memset(zc, 0, sizeof(double) * n8);
+    for (int p = 0; p < Npoly; p++) {
+      const double *Zp = Z + n8 * ((size_t)ci * Npoly + p);
+      const double bp = Bb[p];
+      for (size_t i = 0; i < n8; i++) zc[i] += bp * Zp[i];
+    }
+  }
+}
+
+// The host lines that run after the bands of one minibatch are fitted, decision for decision, with
+// the driver's quirks (DESIGN.md 7): res_0 / res_1 become (previous + sum over bands) / nsolbw, a
+// running mixture; a band is flagged when its cost after the fit exceeds 1.5 res_1 (a cost that is not
+// > 0 counts as CLM_DBL_MAX); good bands get Y_b += rho_b J_b; the sum z = sum_b B_b (x) Y_b always
+// holds band 0, flagged or not; Z = Bi z (update_global_z_multi, consensus_poly.c:706-832); good
+// bands get Y_b -= rho_b B_b Z.
+extern "C" int dirac_b200_consensus_bands_update(int N, int Mt, int nsolbw, int Npoly,
+                                                 const double *res_00, const double *res_01,
+                                                 const double *pfreq, const double *B,
+                                                 const double *Bi, const double *rhok, double *res_0,
+                                                 double *res_1, double *Y, double *Z, int *fband) {
+  if (N < 1 || Mt < 1 || nsolbw < 1 || Npoly < 1) {
+    fprintf(stderr, "dirac_b200_consensus_bands_update: N = %d, Mt = %d, nsolbw = %d, Npoly = %d; "
+                    "each must be at least 1\n", N, Mt, nsolbw, Npoly);
+    return -1;
+  }
+  const size_t n8 = (size_t)8 * N, m = n8 * Mt;
+  const double res_ratio = 1.5, clm_dbl_max = 1e12;  // minibatch_consensus_mode.cpp:262, CLM_DBL_MAX
+  std::vector<double> resband(nsolbw);
+  for (int b = 0; b < nsolbw; b++) {
+    *res_0 += res_00[b];
+    *res_1 += res_01[b];
+    resband[b] = res_00[b] > 0.0 && res_01[b] > 0.0 ? res_01[b] : clm_dbl_max;
+  }
+  *res_0 /= (double)nsolbw;
+  *res_1 /= (double)nsolbw;
+  for (int b = 0; b < nsolbw; b++) fband[b] = resband[b] > res_ratio * *res_1 ? 1 : 0;
+  // Y_b <- Y_b + rho_b J_b for the good bands
+  for (int b = 0; b < nsolbw; b++) {
+    if (fband[b]) continue;
+    for (int ci = 0; ci < Mt; ci++) {
+      const double r = rhok[(size_t)b * Mt + ci];
+      const double *J = pfreq + (size_t)b * m + n8 * ci;
+      double *y = Y + (size_t)b * m + n8 * ci;
+      for (size_t i = 0; i < n8; i++) y[i] += r * J[i];
+    }
+  }
+  // z[p] = sum_b B_b[p] Y_b, laid out [Npoly][Mt][8N]: band 0 unconditionally (:569-572), the others
+  // when good
+  std::vector<double> z((size_t)Npoly * m);
+  for (int p = 0; p < Npoly; p++)
+    for (size_t i = 0; i < m; i++) z[(size_t)p * m + i] = B[p] * Y[i];
+  for (int b = 1; b < nsolbw; b++) {
+    if (fband[b]) continue;
+    for (int p = 0; p < Npoly; p++) {
+      const double bp = B[(size_t)b * Npoly + p];
+      const double *y = Y + (size_t)b * m;
+      double *zp = z.data() + (size_t)p * m;
+      for (size_t i = 0; i < m; i++) zp[i] += bp * y[i];
+    }
+  }
+  // Z[ci][p] = sum_q Bi[ci][p][q] z[q][ci], Z laid out [Mt][Npoly][8N]
+  for (int ci = 0; ci < Mt; ci++)
+    for (int p = 0; p < Npoly; p++) {
+      double *Zp = Z + n8 * ((size_t)ci * Npoly + p);
+      const double *bi = Bi + ((size_t)ci * Npoly + p) * Npoly;
+      for (size_t i = 0; i < n8; i++) {
+        double s = 0.0;
+        for (int q = 0; q < Npoly; q++) s += bi[q] * z[(size_t)q * m + n8 * ci + i];
+        Zp[i] = s;
+      }
+    }
+  // Y_b <- Y_b - rho_b B_b Z for the good bands
+  std::vector<double> bz(m);
+  for (int b = 0; b < nsolbw; b++) {
+    if (fband[b]) continue;
+    db_consensus_bz(Z, B + (size_t)b * Npoly, N, Mt, Npoly, bz.data());
+    for (int ci = 0; ci < Mt; ci++) {
+      const double r = rhok[(size_t)b * Mt + ci];
+      double *y = Y + (size_t)b * m + n8 * ci;
+      for (size_t i = 0; i < n8; i++) y[i] += -r * bz[n8 * ci + i];
+    }
   }
   return 0;
 }

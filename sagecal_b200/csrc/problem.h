@@ -213,5 +213,8 @@ void db_band_fit(BandDev *bd, const BandView &b, double *p, const double *y, con
                  const double *rho, int max_lbfgs, int lbfgs_m, double robust_nu, double *res_0,
                  double *res_1, persistent_data_t *indata);
 
+// z = B_b Z of every chunk (consensus.cu): Z [Mt][Npoly][8N], Bb the band's Npoly basis values, z [Mt][8N]
+void db_consensus_bz(const double *Z, const double *Bb, int N, int Mt, int Npoly, double *z);
+
 void db_lm_free(dirac_b200_problem *pr);
 void db_rtr_free(dirac_b200_problem *pr);

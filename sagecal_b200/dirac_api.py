@@ -524,6 +524,62 @@ class DiracAPI:
             robust_nu, C.cast(pt, C.c_void_p), dptr(pfreq), ccid, rho, phase_only, dptr(r0), dptr(r1))
         return rv, r0, r1
 
+    def stochastic_consensus_interval(self, u, v, w, xo, N, Nbase, tmb, barr, sky: SkyModel, freqs,
+                                      deltaf, pt, pfreq, nsolbw, nepochs, nadmm, B, Bi, rhok, Z,
+                                      use_global=0, uvmin=0.0, uvmax=1e9, max_lbfgs=4, lbfgs_m=5,
+                                      robust_nu=2.0, ccid=-99999, rho=1e-9, phase_only=0):
+        """dirac_b200_stochastic_consensus_interval: the consensus minibatch driver's loop over one
+        interval in one call.  Arguments as stochastic_interval, plus B [nsolbw, Npoly],
+        Bi [Mt, Npoly, Npoly], rhok [nsolbw, Mt] and Z [Mt, Npoly, 8N] (in place).  returns
+        (retval, res_00, res_01 [nadmm, nepochs, minibatches, nsolbw], res_0, res_1, fband [nsolbw])"""
+        L = self.lib
+        dp, i, d = c_double_p, C.c_int, C.c_double
+        L.dirac_b200_stochastic_consensus_interval.restype = i
+        L.dirac_b200_stochastic_consensus_interval.argtypes = [dp] * 4 + [i] * 4 + [
+            C.POINTER(baseline_t), C.POINTER(clus_source_t), i, i, dp, i, d, d, d, i, i, i, i, d,
+            C.c_void_p, dp, i, d, i, i, i, dp, dp, dp, dp, i, dp, dp, dp, dp, c_int_p]
+        for a in (u, v, w, xo, pfreq, Z):
+            assert a.dtype == np.float64 and a.flags.c_contiguous
+        freqs = np.ascontiguousarray(freqs, dtype=np.float64)
+        B = np.ascontiguousarray(B, dtype=np.float64)
+        Bi = np.ascontiguousarray(Bi, dtype=np.float64)
+        rhok = np.ascontiguousarray(rhok, dtype=np.float64)
+        nmb = u.shape[0]
+        r00 = np.zeros((nadmm, nepochs, nmb, nsolbw))
+        r01 = np.zeros((nadmm, nepochs, nmb, nsolbw))
+        r0, r1 = C.c_double(0.0), C.c_double(0.0)
+        fband = np.zeros(max(nsolbw, 1), dtype=np.int32)
+        rv = L.dirac_b200_stochastic_consensus_interval(
+            dptr(u), dptr(v), dptr(w), dptr(xo), N, Nbase, tmb, nmb, barr, sky.arr, sky.M, sky.Mt,
+            dptr(freqs), len(freqs), deltaf, uvmin, uvmax, nsolbw, nepochs, max_lbfgs, lbfgs_m,
+            robust_nu, C.cast(pt, C.c_void_p), dptr(pfreq), ccid, rho, phase_only, nadmm, B.shape[1],
+            dptr(B), dptr(Bi), dptr(rhok), dptr(Z), use_global, dptr(r00), dptr(r01), C.byref(r0),
+            C.byref(r1), fband.ctypes.data_as(c_int_p))
+        return rv, r00, r01, r0.value, r1.value, fband[:nsolbw]
+
+    def consensus_bands_update(self, N, res_00, res_01, pfreq, B, Bi, rhok, res_0, res_1, Y, Z):
+        """dirac_b200_consensus_bands_update: the ADMM step after the bands of one minibatch.
+        pfreq, Y [nsolbw, 8 N Mt]; B [nsolbw, Npoly]; Bi [Mt, Npoly, Npoly]; rhok [nsolbw, Mt];
+        Z [Mt, Npoly, 8N].  Y and Z in place; returns (retval, res_0, res_1, fband)"""
+        L = self.lib
+        dp = c_double_p
+        L.dirac_b200_consensus_bands_update.restype = C.c_int
+        L.dirac_b200_consensus_bands_update.argtypes = [C.c_int] * 4 + [dp] * 6 + [dp, dp, dp, dp,
+                                                                                 c_int_p]
+        nsolbw, Npoly = B.shape
+        Mt = Bi.shape[0]
+        for a in (Y, Z):
+            assert a.dtype == np.float64 and a.flags.c_contiguous
+        r00 = np.ascontiguousarray(res_00, dtype=np.float64)
+        r01 = np.ascontiguousarray(res_01, dtype=np.float64)
+        args = [np.ascontiguousarray(a, dtype=np.float64) for a in (pfreq, B, Bi, rhok)]
+        r0, r1 = C.c_double(res_0), C.c_double(res_1)
+        fband = np.zeros(max(nsolbw, 1), dtype=np.int32)
+        rv = L.dirac_b200_consensus_bands_update(N, Mt, nsolbw, Npoly, dptr(r00), dptr(r01),
+                                                 *[dptr(a) for a in args], C.byref(r0), C.byref(r1),
+                                                 dptr(Y), dptr(Z), fband.ctypes.data_as(c_int_p))
+        return rv, r0.value, r1.value, fband[:nsolbw]
+
     def persist_init_array(self, nbands, nminibatch, m, n, lbfgs_m, Nt=4):
         """nbands persistent_data_t of include/dirac_b200.h back to back, as the driver's
         ptdata_array, each initialised by lbfgs_persist_init"""

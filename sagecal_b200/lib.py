@@ -52,8 +52,10 @@ DIFFUSE_EXPORTED = ["recalculate_diffuse_coherencies", "dirac_b200_diffuse_coher
 #: every symbol include/dirac_b200_channels.h declares (per-channel refinement, driver option -b 1)
 CHANNELS_EXPORTED = ["calculate_residuals", "dirac_b200_bfgsfit_channels", "dirac_b200_transfer_stats"]
 
-#: every symbol include/dirac_b200_stochastic.h declares (stochastic calibration of an interval)
-STOCHASTIC_EXPORTED = ["dirac_b200_stochastic_interval"]
+#: every symbol include/dirac_b200_stochastic.h declares (stochastic calibration of an interval, with
+#: or without spectral consensus over the bands)
+STOCHASTIC_EXPORTED = ["dirac_b200_stochastic_interval", "dirac_b200_stochastic_consensus_interval",
+                       "dirac_b200_consensus_bands_update"]
 
 
 class DiracB200(DiracAPI):
