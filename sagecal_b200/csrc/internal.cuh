@@ -318,27 +318,20 @@ struct GramArgs {
   int t_begin, t_end, t_step;  // timeslots t_begin, t_begin+t_step, ... < t_end
 };
 
+// J^T J of one system, or of a batch (matrix y of the batch belongs to local cluster list[y]).
+// Baseline b of the station pair p < q is the b-th pair in (p, q) lexicographic order (problem.cu).
 struct AssembleArgs {
-  const double *T;       // [Nbase][16] Gram tensors of this cluster / time range
-  const double *pblk;    // 8N Jones
-  double *JTJ;           // [8N][8N]
-  double *Hst;           // [N][4] station sums (H00, H11, Re H01, Im H01), zeroed by the caller
-  const TileDesc *tiles;
-  const short2 *blpq;    // [Nbase] (p,q) of baseline b
-  int N, Nbase;
-};
-
-// all (eligible) clusters of a sweep at once: matrix y of the batch belongs to local cluster list[y]
-struct BatchAssembleArgs {
-  const double *T;       // Gram tensors [Mt][Nbase][16]
-  const double *pp;      // device Jones vector
-  const int *list;       // [nb] local cluster indices
-  const int *tix;        // [M] Gram slot of cluster k (first chunk)
-  const int *poff;       // [M] offset of cluster k's (first) block in pp
-  double *JTJ;           // [nb][8N][8N]
-  double *Hst;           // [nb][N][4], zeroed by the caller
-  const TileDesc *tiles;
-  const short2 *blpq;    // [Nbase] (p,q) of baseline b
+  const double *T;       // [Nbase][16] Gram tensors; batch: [Mt][Nbase][16], slot tix[list[y]]
+  const double *pblk;    // 8N Jones; batch: the Jones vector, cluster block at poff[list[y]]
+  const int *list;       // batch: [nb] local cluster indices; null: one system
+  const int *tix;        // batch: [M] Gram slot of cluster k (first chunk)
+  const int *poff;       // batch: [M] offset of cluster k's (first) block in pblk
+  double *JTJ;           // [8N][8N]; batch: matrix y at JTJ + y * stride
+  long long stride;
+  double *Hst;           // [N][4] station sums (H00, H11, Re H01, Im H01); batch: [nb][N][4]
+  const double *mu_dev;  // batch: damping of matrix y; null: mu
+  double mu;             // added to the diagonal
+  int lower;             // 1: write only the lower triangle (column-major) and the diagonal
   int N, Nbase;
 };
 
@@ -374,7 +367,9 @@ void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st
 // forms the hidden data itself (ClusterPassArgs::form_hidden)
 int db_cluster_pass_forms_hidden(int N, int Nbase);
 void db_launch_coh_gram(const GramArgs *a, int ntile, int nk, cudaStream_t st);
-void db_launch_assemble(const AssembleArgs *a, int ntile, cudaStream_t st);
+void db_launch_station_sums(const AssembleArgs *a, int nb, cudaStream_t st);
+void db_launch_assemble_tiles(const AssembleArgs *a, int nb, cudaStream_t st);
+void db_launch_batch_mu0(const double *Hst, double *mu, int N, double tau, int nb, cudaStream_t st);
 void db_launch_copy_add_diag(const double *A0, double *A, int n, double mu, cudaStream_t st);
 // kernels_chol.cu: (A + mu I) x = b on one thread-block cluster
 int db_chol_max_n();

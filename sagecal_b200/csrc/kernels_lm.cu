@@ -27,144 +27,165 @@ struct Gram {
 };
 
 
-// One baseline's contribution to J^T J.  The 16 2x2 sub-blocks of the (p,q) coupling (and their
-// mirror images) are shared out over 16 threads (`sub`): each thread recomputes the few hundred flops
-// (indices stay static, everything in registers) and writes only its own 8 entries, so the scattered
-// stores of a baseline are spread over 16 threads and the grid has Nbase*16 threads instead of 13 CTAs.
-__device__ __forceinline__ void assemble_baseline(const AssembleArgs &a, int p, int q, long long b,
-                                                  int sub) {
+// Baseline index of the station pair p < q (the canonical order problem.cu builds blpq in)
+__device__ __forceinline__ long long pair_baseline(int p, int q, int N) {
+  return (long long)p * (2 * N - p - 1) / 2 + (q - p - 1);
+}
+
+__device__ __forceinline__ Gram load_gram(const double *T, long long b) {
   Gram G;
-  {
-    const double2 *Tb = reinterpret_cast<const double2 *>(a.T + b * 16);
-    double2 t0 = Tb[0], t1 = Tb[1];
-    G.d[0] = t0.x; G.d[1] = t0.y; G.d[2] = t1.x; G.d[3] = t1.y;
+  const double2 *Tb = reinterpret_cast<const double2 *>(T + b * 16);
+  const double2 t0 = __ldg(Tb), t1 = __ldg(Tb + 1);
+  G.d[0] = t0.x; G.d[1] = t0.y; G.d[2] = t1.x; G.d[3] = t1.y;
 #pragma unroll
-    for (int z = 0; z < 6; z++) G.o[z] = Tb[2 + z];
+  for (int z = 0; z < 6; z++) G.o[z] = __ldg(Tb + 2 + z);
+  return G;
+}
+
+// system y of an assembly launch (one system, or matrix y of a batch over b.list)
+struct AsmSys {
+  const double *T, *J;
+  double *A, *H;
+  double mu;
+};
+__device__ __forceinline__ AsmSys asm_sys(const AssembleArgs &a, int y) {
+  AsmSys s;
+  if (a.list) {
+    const int k = a.list[y];
+    s.T = a.T + (long long)a.tix[k] * a.Nbase * 16;
+    s.J = a.pblk + a.poff[k];
+  } else {
+    s.T = a.T;
+    s.J = a.pblk;
   }
-  double2 Jp[4], Jq[4];
-  load_jones(a.pblk, p, Jp);
-  load_jones(a.pblk, q, Jq);
-  const int ld = 8 * a.N;
-  // cross block
-#pragma unroll
-  for (int i = 0; i < 2; i++)
+  s.A = a.JTJ + (long long)y * a.stride;
+  s.H = a.Hst + (long long)y * 4 * a.N;
+  s.mu = a.mu_dev ? a.mu_dev[y] : a.mu;
+  return s;
+}
+
+// Station sums of the diagonal blocks: one warp per station s walks its N-1 baselines (lane-strided)
+// and reduces with a fixed shuffle tree, so the sums do not depend on scheduling.
+//   s = p of (s,o):  Hp_ll' = sum_ab (Jo^H Jo)_ab Th[(l',b),(l,a)]
+//   s = q of (o,s):  Hq_ll' = sum_ab (Jo^H Jo)_ab Th[(a,l),(b,l')]
+// Hst[s] = (H00, H11, Re H01, Im H01); blockIdx.y: matrix of the batch.
+__global__ void __launch_bounds__(256)
+k_station_sums(AssembleArgs a) {
+  const AsmSys S = asm_sys(a, blockIdx.y);
+  const int s = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (s >= a.N) return;
+  double h0 = 0.0, h1 = 0.0, h2 = 0.0, h3 = 0.0;
+  for (int o = lane; o < a.N; o += 32) {
+    if (o == s) continue;
+    const bool sp = s < o;
+    const Gram G = load_gram(S.T, sp ? pair_baseline(s, o, a.N) : pair_baseline(o, s, a.N));
+    double2 Jo[4], Qo[4];
+    load_jones(S.J, o, Jo);
+    mat_ahb(Jo, Jo, Qo);
+    double2 h[4];
 #pragma unroll
     for (int l = 0; l < 2; l++)
 #pragma unroll
-      for (int j = 0; j < 2; j++)
+      for (int lp = 0; lp < 2; lp++) {
+        double2 z = make_double2(0.0, 0.0);
 #pragma unroll
-        for (int lp = 0; lp < 2; lp++) {
-          double2 z = make_double2(0.0, 0.0);
+        for (int aa = 0; aa < 2; aa++)
 #pragma unroll
-          for (int aa = 0; aa < 2; aa++)
+          for (int bb = 0; bb < 2; bb++)
+            cfma(z, Qo[2 * aa + bb], sp ? G.at(2 * lp + bb, 2 * l + aa) : G.at(2 * aa + l, 2 * bb + lp));
+        h[2 * l + lp] = z;
+      }
+    h0 += h[0].x;
+    h1 += h[3].x;
+    h2 += h[1].x;
+    h3 += h[1].y;
+  }
+  h0 = warp_sum(h0);
+  h1 = warp_sum(h1);
+  h2 = warp_sum(h2);
+  h3 = warp_sum(h3);
+  if (lane == 0) {
+    S.H[4 * s] = h0;
+    S.H[4 * s + 1] = h1;
+    S.H[4 * s + 2] = h2;
+    S.H[4 * s + 3] = h3;
+  }
+}
+
+// J^T J (+ mu I) by output tiles.  Memory row R = 8P + r holds, from column 8Q on, the 8x8 block of
+// the station pair (P,Q).  A warp owns station P and a group of 8 stations Q: lane t computes the 2x2
+// sub-blocks (i,l) x (j,lp) = (0..3) x (t & 3) of the pair (P, Q0 + t/4) and stores them as double2,
+// so each store of the warp is one contiguous 512-byte row segment.  A CTA (8 warps) covers 64
+// stations Q of one station P; blockIdx.z: matrix of the batch.
+//
+// `lower`: only the Q groups that reach Q >= P are written, i.e. the lower triangle of the
+// column-major matrix that dpotrf(LOWER) and the blocked triangular solves read (plus a few blocks
+// of the other triangle in the diagonal group, written with their true values).
+//
+// Off-diagonal block (p,q), p < q: [(i,l),(j,l')] = R(z) S = [[zr, zi],[zi, -zr]] with
+// z = sum_ab Jq_ja Jp_ib Th[(l,a),(b,l')]; the 2x2 is symmetric, so block (q,p) holds the same 2x2
+// at the transposed sub-block.  Diagonal block: the station sums (k_station_sums) plus mu.
+__global__ void __launch_bounds__(256)
+k_assemble_tiles(AssembleArgs a) {
+  const int P = blockIdx.x;
+  const int qcta = blockIdx.y * 64;
+  if (a.lower && qcta + 64 <= P) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = qcta + 8 * warp;
+  if (q0 >= a.N || (a.lower && q0 + 8 <= P)) return;
+  const AsmSys S = asm_sys(a, blockIdx.z);
+  const int Q = q0 + (lane >> 2);
+  const int jl = lane & 3, j = jl >> 1, lp = jl & 1;
+  const long long ld = 8ll * a.N;
+  if (Q == P) {
+    const double h00 = S.H[4 * P], h11 = S.H[4 * P + 1], hr = S.H[4 * P + 2], hi = S.H[4 * P + 3];
+    // 4x4 block of polarisation row i = column j; the blocks i != j are zero
+    const double blk[4][4] = {{h00, 0.0, hr, hi}, {0.0, h00, -hi, hr}, {hr, -hi, h11, 0.0},
+                              {hi, hr, 0.0, h11}};
 #pragma unroll
-            for (int bb = 0; bb < 2; bb++) {
-              double2 jj = cmul(Jq[2 * j + aa], Jp[2 * i + bb]);
-              cfma(z, jj, G.at(2 * l + aa, 2 * bb + lp));
-            }
-          if (sub != ((i * 2 + l) * 2 + j) * 2 + lp) continue;
-          const int r0 = 8 * p + 2 * (2 * i + l);
-          const int c0 = 8 * q + 2 * (2 * j + lp);
-          // R(z) S = [[zr, zi],[zi, -zr]]
-          a.JTJ[(long long)r0 * ld + c0] = z.x;
-          a.JTJ[(long long)r0 * ld + c0 + 1] = z.y;
-          a.JTJ[(long long)(r0 + 1) * ld + c0] = z.y;
-          a.JTJ[(long long)(r0 + 1) * ld + c0 + 1] = -z.x;
-          // transposed block (q,p)
-          a.JTJ[(long long)c0 * ld + r0] = z.x;
-          a.JTJ[(long long)(c0 + 1) * ld + r0] = z.y;
-          a.JTJ[(long long)c0 * ld + r0 + 1] = z.y;
-          a.JTJ[(long long)(c0 + 1) * ld + r0 + 1] = -z.x;
-        }
-  // diagonal contributions
-  double2 Qq[4], Qp[4];
-  mat_ahb(Jq, Jq, Qq);
-  mat_ahb(Jp, Jp, Qp);
-  double2 Hp[4], Hq[4];
+    for (int il = 0; il < 4; il++) {
+      const int i = il >> 1, l = il & 1;
+      double2 v0 = make_double2(0.0, 0.0), v1 = v0;
+      if (i == j) {  // (lane-dependent lp selects between static indices: no local memory)
+        const double m = (l == lp) ? S.mu : 0.0;
+        v0 = lp ? make_double2(blk[2 * l][2], blk[2 * l][3]) : make_double2(blk[2 * l][0], blk[2 * l][1]);
+        v1 = lp ? make_double2(blk[2 * l + 1][2], blk[2 * l + 1][3])
+                : make_double2(blk[2 * l + 1][0], blk[2 * l + 1][1]);
+        v0.x += m;
+        v1.y += m;
+      }
+      const long long r0 = 8ll * P + 2 * il;
+      *reinterpret_cast<double2 *>(S.A + r0 * ld + 8ll * Q + 2 * jl) = v0;
+      *reinterpret_cast<double2 *>(S.A + (r0 + 1) * ld + 8ll * Q + 2 * jl) = v1;
+    }
+    return;
+  }
+  if (Q < a.N) {
+    const bool pq = P < Q;  // the pair's baseline is (P,Q); otherwise (Q,P) and its block transposed
+    const Gram G = load_gram(S.T, pq ? pair_baseline(P, Q, a.N) : pair_baseline(Q, P, a.N));
+    double2 JP[4], JQ[4];
+    load_jones(S.J, P, JP);
+    load_jones(S.J, Q, JQ);
+    const double2 Jj[2] = {j ? JQ[2] : JQ[0], j ? JQ[3] : JQ[1]};  // JQ[2j + x]
 #pragma unroll
-  for (int l = 0; l < 2; l++)
-#pragma unroll
-    for (int lp = 0; lp < 2; lp++) {
-      double2 hp = make_double2(0.0, 0.0), hq = make_double2(0.0, 0.0);
+    for (int il = 0; il < 4; il++) {
+      const int i = il >> 1, l = il & 1;
+      double2 z = make_double2(0.0, 0.0);
 #pragma unroll
       for (int aa = 0; aa < 2; aa++)
 #pragma unroll
         for (int bb = 0; bb < 2; bb++) {
-          cfma(hp, Qq[2 * aa + bb], G.at(2 * lp + bb, 2 * l + aa));
-          cfma(hq, Qp[2 * aa + bb], G.at(2 * aa + l, 2 * bb + lp));
+          if (pq)  // baseline (p,q) = (P,Q), sub-block (i,l) x (j,lp)
+            cfma(z, cmul(Jj[aa], JP[2 * i + bb]),
+                 lp ? G.at(2 * l + aa, 2 * bb + 1) : G.at(2 * l + aa, 2 * bb));
+          else     // baseline (p,q) = (Q,P), sub-block (j,lp) x (i,l)
+            cfma(z, cmul(JP[2 * i + aa], Jj[bb]), lp ? G.at(2 + aa, 2 * bb + l) : G.at(aa, 2 * bb + l));
         }
-      Hp[2 * l + lp] = hp;
-      Hq[2 * l + lp] = hq;
+      const long long r0 = 8ll * P + 2 * il;
+      *reinterpret_cast<double2 *>(S.A + r0 * ld + 8ll * Q + 2 * jl) = z;
+      *reinterpret_cast<double2 *>(S.A + (r0 + 1) * ld + 8ll * Q + 2 * jl) = make_double2(z.y, -z.x);
     }
-  if (sub == 0) atomicAdd(a.Hst + 4 * p + 0, Hp[0].x);
-  if (sub == 1) atomicAdd(a.Hst + 4 * p + 1, Hp[3].x);
-  if (sub == 2) atomicAdd(a.Hst + 4 * p + 2, Hp[1].x);
-  if (sub == 3) atomicAdd(a.Hst + 4 * p + 3, Hp[1].y);
-  if (sub == 4) atomicAdd(a.Hst + 4 * q + 0, Hq[0].x);
-  if (sub == 5) atomicAdd(a.Hst + 4 * q + 1, Hq[3].x);
-  if (sub == 6) atomicAdd(a.Hst + 4 * q + 2, Hq[1].x);
-  if (sub == 7) atomicAdd(a.Hst + 4 * q + 3, Hq[1].y);
-}
-
-// thread -> (baseline, sub-block): 16 consecutive threads share a baseline
-__device__ __forceinline__ void assemble_lin(const AssembleArgs &a) {
-  const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long b = gid >> 4;
-  if (b >= a.Nbase) return;
-  const short2 pq = a.blpq[b];
-  assemble_baseline(a, pq.x, pq.y, b, (int)(gid & 15));
-}
-
-__global__ void __launch_bounds__(256)
-k_assemble_offdiag(AssembleArgs a) {
-  assemble_lin(a);
-}
-
-// batched over clusters (blockIdx.y): all normal matrices of a SAGE sweep in one launch
-__global__ void __launch_bounds__(256)
-k_assemble_offdiag_batched(BatchAssembleArgs b) {
-  const int k = b.list[blockIdx.y];
-  AssembleArgs a;
-  a.T = b.T + (long long)b.tix[k] * b.Nbase * 16;
-  a.pblk = b.pp + b.poff[k];
-  a.JTJ = b.JTJ + (long long)blockIdx.y * 64 * b.N * b.N;
-  a.Hst = b.Hst + (long long)blockIdx.y * 4 * b.N;
-  a.tiles = b.tiles;
-  a.blpq = b.blpq;
-  a.N = b.N;
-  a.Nbase = b.Nbase;
-  assemble_lin(a);
-}
-
-__device__ __forceinline__ void assemble_diag_station(const double *__restrict__ Hst,
-                                                      double *__restrict__ JTJ, int N, int s);
-
-// diagonal 8x8 blocks from the station sums; one thread per (station, 4x4 sub-block i)
-__global__ void k_assemble_diag(const double *__restrict__ Hst, double *__restrict__ JTJ, int N) {
-  int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= N) return;
-  assemble_diag_station(Hst, JTJ, N, s);
-}
-__global__ void k_assemble_diag_batched(const double *__restrict__ Hst, double *__restrict__ JTJ,
-                                        int N) {
-  int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= N) return;
-  assemble_diag_station(Hst + (long long)blockIdx.y * 4 * N, JTJ + (long long)blockIdx.y * 64 * N * N,
-                        N, s);
-}
-__device__ __forceinline__ void assemble_diag_station(const double *__restrict__ Hst,
-                                                      double *__restrict__ JTJ, int N, int s) {
-  const double h00 = Hst[4 * s], h11 = Hst[4 * s + 1], hr = Hst[4 * s + 2], hi = Hst[4 * s + 3];
-  const int ld = 8 * N;
-  for (int i = 0; i < 2; i++) {
-    double blk[4][4] = {{h00, 0.0, hr, hi}, {0.0, h00, -hi, hr}, {hr, -hi, h11, 0.0},
-                        {hi, hr, 0.0, h11}};
-    for (int r = 0; r < 8; r++)
-      for (int c = 0; c < 8; c++) {
-        double v = 0.0;
-        if ((r >> 2) == i && (c >> 2) == i) v = blk[r & 3][c & 3];
-        if ((r >> 2) == i) JTJ[(long long)(8 * s + r) * ld + 8 * s + c] = v;
-      }
   }
 }
 
@@ -191,18 +212,6 @@ k_batch_mu0(const double *__restrict__ Hst, double *__restrict__ mu, int N, doub
     for (int i = 1; i < 4; i++)
       if (fabs(sv[i]) > fabs(mx)) mx = sv[i];
     mu[blockIdx.x] = tau * mx;
-  }
-}
-
-// A[y] = A0[y] + mu[y] I over a batch of n x n matrices
-__global__ void k_batch_add_diag(const double *__restrict__ A0, double *__restrict__ A,
-                                 const double *__restrict__ mu, int n) {
-  const long long nn = (long long)n * n;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < nn) {
-    double v = A0[(long long)blockIdx.y * nn + i];
-    if (i / n == i % n) v += mu[blockIdx.y];
-    A[(long long)blockIdx.y * nn + i] = v;
   }
 }
 
@@ -277,24 +286,14 @@ void db_launch_lm_step(const double *p, const double *Dp, const double *jte, dou
 void db_launch_extract_diag(const double *A, double *dst, int n, cudaStream_t st) {
   k_extract_diag<<<(n + 127) / 128, 128, 0, st>>>(A, dst, n);
 }
-void db_launch_assemble(const AssembleArgs *a, int ntile, cudaStream_t st) {
-  (void)ntile;
-  k_assemble_offdiag<<<(a->Nbase * 16 + 255) / 256, 256, 0, st>>>(*a);
-  k_assemble_diag<<<(a->N + 63) / 64, 64, 0, st>>>(a->Hst, a->JTJ, a->N);
+void db_launch_station_sums(const AssembleArgs *a, int nb, cudaStream_t st) {
+  k_station_sums<<<dim3((a->N + 7) / 8, nb), 256, 0, st>>>(*a);
 }
-void db_launch_assemble_batched(const BatchAssembleArgs *b, int ntile, int nb, double tau,
-                                double *mu, double *Afac, cudaStream_t st) {
-  (void)ntile;
-  dim3 g1((b->Nbase * 16 + 255) / 256, nb);
-  k_assemble_offdiag_batched<<<g1, 256, 0, st>>>(*b);
-  dim3 g2((b->N + 63) / 64, nb);
-  k_assemble_diag_batched<<<g2, 64, 0, st>>>(b->Hst, b->JTJ, b->N);
-  k_batch_mu0<<<nb, 128, 0, st>>>(b->Hst, mu, b->N, tau);
-  if (!Afac) return;  // the cluster Cholesky reads J^T J and mu itself
-  const int n = 8 * b->N;
-  const long long nn = (long long)n * n;
-  dim3 g3((unsigned)((nn + 255) / 256), nb);
-  k_batch_add_diag<<<g3, 256, 0, st>>>(b->JTJ, Afac, mu, n);
+void db_launch_assemble_tiles(const AssembleArgs *a, int nb, cudaStream_t st) {
+  k_assemble_tiles<<<dim3(a->N, (a->N + 63) / 64, nb), 256, 0, st>>>(*a);
+}
+void db_launch_batch_mu0(const double *Hst, double *mu, int N, double tau, int nb, cudaStream_t st) {
+  k_batch_mu0<<<nb, 128, 0, st>>>(Hst, mu, N, tau);
 }
 void db_launch_copy_add_diag(const double *A0, double *A, int n, double mu, cudaStream_t st) {
   long long nn = (long long)n * n;

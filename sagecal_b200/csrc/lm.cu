@@ -5,7 +5,8 @@
 // osrlevmar_der_single_nocuda (robustlm.c:2607-3250) decision for decision; what differs is how
 // the quantities are produced:
 //   e, ||e||^2, J^T e   one streaming pass over (hidden data, coh_k)          k_cluster_pass
-//   J^T J               assembled from the per-baseline Gram tensors           k_coh_gram/k_assemble
+//   J^T J               assembled from the per-baseline Gram tensors           k_coh_gram/
+//                       (8N > 512: damped, lower triangle, factored in place)  k_assemble_tiles
 //                       (weighted, robust LM: one streaming pass)              k_weighted_jtj
 //   (J^T J + mu I) dp   linsolv 0: k_chol_solve / k_tri_solve on one thread-block cluster
 //                       (kernels_chol.cu; cuSOLVER potrf/potrs when 8N > 512 or no cluster)
@@ -46,8 +47,6 @@ void db_launch_update_weights(const double2 *e, double2 *wt, long long R, long l
 void db_launch_scale_vis(double2 *v, long long R, long long r0, long long r1, double alpha,
                          int set_const, cudaStream_t st);
 void db_launch_extract_diag(const double *A, double *dst, int n, cudaStream_t st);
-void db_launch_assemble_batched(const BatchAssembleArgs *b, int ntile, int nb, double tau,
-                                double *mu, double *Afac, cudaStream_t st);
 void db_launch_lm_step(const double *p, const double *Dp, const double *jte, double *pnew,
                        double *sc, double *zero, int n, cudaStream_t st);
 void db_launch_os_shift(const double2 *e, const double2 *wt, double2 *eps, double2 *wout, long long R,
@@ -85,6 +84,7 @@ void db_lm_init(dirac_b200_problem *pr) {
   w.os_eps = w.os_w = nullptr;
   w.HP = w.HQ = nullptr;
   w.JB = w.LB = nullptr;
+  w.sys_T = w.sys_p = w.sys_H = nullptr;
   w.pref_slot = (int *)malloc(sizeof(int) * d.M);
   for (int k = 0; k < d.M; k++) w.pref_slot[k] = -1;
   w.jtj0_cur = nullptr;
@@ -162,8 +162,9 @@ void db_lm_free(dirac_b200_problem *pr) {
   if (w.svdS) { db_free(w.svdS); db_free(w.svdU); db_free(w.svdVT); }
   if (w.wbuf) { db_free(w.wbuf); db_free(w.ebuf); db_free(w.HP); db_free(w.HQ); }
   if (w.os_eps) { db_free(w.os_eps); db_free(w.os_w); }
-  if (w.JB) {
-    db_free(w.JB); db_free(w.LB); db_free(w.HB); db_free(w.mu_dev); db_free(w.binfo_dev);
+  if (w.LB) {
+    if (w.JB) db_free(w.JB);
+    db_free(w.LB); db_free(w.HB); db_free(w.mu_dev); db_free(w.binfo_dev);
     db_free(w.LBptr_dev); db_free(w.blist_dev); db_free(w.btix_dev); db_free(w.bpoff_dev);
     cudaFreeHost(w.h_mu); cudaFreeHost(w.h_binfo);
   }
@@ -239,19 +240,44 @@ static void gram(dirac_b200_problem *pr, int k, int t0, int t1, int step, double
   db_count_launch(1);
 }
 
+static AssembleArgs assemble_args(const DevProblem &d, const double *T, const double *pblk_dev,
+                                  double *Hst) {
+  AssembleArgs a;
+  memset(&a, 0, sizeof(a));
+  a.T = T; a.pblk = pblk_dev; a.Hst = Hst; a.N = d.N; a.Nbase = d.Nbase;
+  return a;
+}
+
+// station sums of the diagonal blocks of nb systems (each reads its Gram tensors twice)
+static void station_sums(dirac_b200_problem *pr, const AssembleArgs &a, int nb) {
+  DevProblem &d = pr->d;
+  db_prof_begin(4, nb * 256.0 * d.Nbase, d.stream);
+  db_launch_station_sums(&a, nb, d.stream);
+  db_prof_end(d.stream);
+  db_count_launch(1);
+}
+
+// the matrices of nb systems from their station sums: full, or (lower) the lower triangle and the
+// diagonal only, each Gram tensor read once
+static void assemble_tiles(dirac_b200_problem *pr, const AssembleArgs &a, int nb) {
+  DevProblem &d = pr->d;
+  const double n = 8.0 * d.N;
+  db_prof_begin(4, nb * (a.lower ? 128.0 * d.Nbase + 4.0 * n * (n + 1) : 256.0 * d.Nbase + 8.0 * n * n),
+                d.stream);
+  db_launch_assemble_tiles(&a, nb, d.stream);
+  db_prof_end(d.stream);
+  db_count_launch(1);
+}
+
+// J^T J at pblk_dev from the Gram tensors T: station sums into w.Hst, then the full undamped matrix
+// into JTJ (JTJ == null: the station sums only; the solve writes the damped matrix, enqueue_solve)
 static void assemble(dirac_b200_problem *pr, const double *T, const double *pblk_dev,
                      double *JTJ) {
-  DevProblem &d = pr->d;
-  LMWork &w = pr->lm;
-  DB_CHECK(cudaMemsetAsync(w.Hst, 0, sizeof(double) * 4 * d.N, d.stream));
-  AssembleArgs a;
-  a.T = T; a.pblk = pblk_dev; a.JTJ = JTJ; a.Hst = w.Hst; a.tiles = d.tiles; a.blpq = d.blpq;
-  a.N = d.N;
-  a.Nbase = d.Nbase;
-  db_prof_begin(4, 128.0 * d.Nbase + 8.0 * 64.0 * d.N * d.N, d.stream);
-  db_launch_assemble(&a, d.ntile, d.stream);
-  db_prof_end(d.stream);
-  db_count_launch(2);
+  AssembleArgs a = assemble_args(pr->d, T, pblk_dev, pr->lm.Hst);
+  station_sums(pr, a, 1);
+  if (!JTJ) return;
+  a.JTJ = JTJ;
+  assemble_tiles(pr, a, 1);
 }
 
 // weighted J^T J of cluster k over timeslots [t0,t1) by streaming (robust LM)
@@ -314,8 +340,20 @@ static int enqueue_solve(dirac_b200_problem *pr, double mu, int linsolv, double 
     w.step_fused = w.step_armed;  // the kernel's epilogue formed the trial point (db_chol_set_step)
     return 1;
   }
-  db_launch_copy_add_diag(w.jtj0_cur ? w.jtj0_cur : w.JTJ0, w.JTJ, n, mu, d.stream);
-  db_count_launch(1);
+  if (linsolv == 0 && w.sys_T) {
+    // the lower triangle of J^T J + mu I straight from the Gram tensors into the buffer dpotrf factors
+    // in place: a system rejected at this mu is rebuilt the same way at the next one
+    AssembleArgs a = assemble_args(d, w.sys_T, w.sys_p, const_cast<double *>(w.sys_H));
+    a.JTJ = w.JTJ;
+    a.mu = mu;
+    a.lower = 1;
+    assemble_tiles(pr, a, 1);
+  } else {
+    db_prof_begin(4, 16.0 * n * n, d.stream);
+    db_launch_copy_add_diag(w.jtj0_cur ? w.jtj0_cur : w.JTJ0, w.JTJ, n, mu, d.stream);
+    db_prof_end(d.stream);
+    db_count_launch(1);
+  }
   DB_CHECK(cudaMemcpyAsync(w.Dp, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToDevice, d.stream));
   db_prof_begin(5, 0.0, d.stream);
   if (linsolv == 0) {
@@ -393,15 +431,19 @@ void db_prefactor_sweep(dirac_b200_problem *pr, double tau) {
   LMWork &w = pr->lm;
   const int n = w.n8;
   const size_t nn = (size_t)n * n;
-  if ((double)d.M * nn * 16.0 > 24e9) return;  // keep the two batch buffers within 24 GB
   // own batched factorisation (one 16-CTA cluster per matrix) when the cluster solver takes the size:
   // the factor of cluster b then lives in a k_chol_solve workspace (ld = 32*ceil(n/32))
   const bool own_batch = w.own_chol && db_tri_available(n) && !getenv("DIRAC_B200_BATCH_CUSOLVER");
+  // The cluster solvers read the undamped J^T J (JB) and damp it themselves.  cuSOLVER factors the
+  // lower triangle of J^T J + mu0 I written straight into LB, in place; a rejected first step is
+  // re-assembled from the Gram tensors (enqueue_solve), so no undamped copy is kept.
+  const bool keep_jb = w.own_chol;
+  if ((double)d.M * nn * 8.0 * (keep_jb ? 2 : 1) > 24e9) return;  // batch buffers within 24 GB
   const size_t lstride = own_batch ? db_chol_ws_doubles(n) : nn;
   w.lb_stride = lstride;
   w.lb_ld = own_batch ? 32 * ((n + 31) / 32) : n;
-  if (!w.JB) {
-    w.JB = dalloc<double>(nn * d.M);
+  if (!w.LB) {
+    w.JB = keep_jb ? dalloc<double>(nn * d.M) : nullptr;
     w.LB = dalloc<double>(lstride * d.M);
     w.HB = dalloc<double>((size_t)4 * d.N * d.M);
     w.mu_dev = dalloc<double>(d.M);
@@ -458,14 +500,24 @@ void db_prefactor_sweep(dirac_b200_problem *pr, double tau) {
   if (nb == 0) return;
   DB_CHECK(cudaMemcpyAsync(w.blist_dev, list.data(), sizeof(int) * nb, cudaMemcpyHostToDevice,
                            d.stream));
-  DB_CHECK(cudaMemsetAsync(w.HB, 0, sizeof(double) * 4 * d.N * nb, d.stream));
-  BatchAssembleArgs b;
-  b.T = w.T; b.pp = d.pp; b.list = w.blist_dev; b.tix = w.btix_dev; b.poff = w.bpoff_dev;
-  b.JTJ = w.JB; b.Hst = w.HB; b.tiles = d.tiles; b.blpq = d.blpq; b.N = d.N; b.Nbase = d.Nbase;
-  db_prof_begin(4, nb * (128.0 * d.Nbase + 8.0 * 64.0 * d.N * d.N), d.stream);
-  db_launch_assemble_batched(&b, d.ntile, nb, tau, w.mu_dev, own_batch ? nullptr : w.LB, d.stream);
-  db_prof_end(d.stream);
-  db_count_launch(4);
+  AssembleArgs b = assemble_args(d, w.T, d.pp, w.HB);
+  b.list = w.blist_dev; b.tix = w.btix_dev; b.poff = w.bpoff_dev;
+  station_sums(pr, b, nb);
+  // mu0 = tau * max_i (J^T J)_ii (clmfit.c:342-352) of every matrix, from the station sums
+  db_launch_batch_mu0(w.HB, w.mu_dev, d.N, tau, nb, d.stream);
+  db_count_launch(1);
+  if (keep_jb) {
+    b.JTJ = w.JB;
+    b.stride = (long long)nn;
+    assemble_tiles(pr, b, nb);
+  }
+  if (!own_batch) {
+    b.JTJ = w.LB;
+    b.stride = (long long)lstride;
+    b.mu_dev = w.mu_dev;
+    b.lower = 1;
+    assemble_tiles(pr, b, nb);
+  }
   db_prof_begin(5, 0.0, d.stream);
   if (own_batch) {
     db_launch_chol_factor_batched(w.JB, n, w.mu_dev, w.LB, (long long)lstride, w.binfo_dev, nb,
@@ -784,7 +836,12 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
       const int slot = (!wt && !os && kiter == 0 && linsolv == 0) ? w.pref_slot[k] : -1;
       const bool prefac = slot >= 0;
       const bool need_mx = (kiter == 0) && !prefac;
-      w.jtj0_cur = prefac ? w.JB + (size_t)slot * n * n : nullptr;
+      w.jtj0_cur = (prefac && w.JB) ? w.JB + (size_t)slot * n * n : nullptr;
+      // unweighted systems of the cuSOLVER Cholesky: each solve assembles J^T J + mu I itself
+      const bool in_place = !w.own_chol && linsolv == 0 && !wt && !os;
+      w.sys_T = in_place ? Tfull : nullptr;
+      w.sys_p = pblk_dev;
+      w.sys_H = prefac ? w.HB + (size_t)slot * 4 * d.N : w.Hst;
       if (os) {
         const int l = randomize ? subI[ositer] : (os_shift + kiter + ositer) % Nsubsets;
         os_subset_system(pr, k, t0, t1, l, pblk_dev, wt);
@@ -799,7 +856,7 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
         w.jtj0_cur = w.jtj_spec;
         w.jtj_spec = nullptr;
       } else {
-        assemble(pr, Tfull, pblk_dev, w.JTJ0);
+        assemble(pr, Tfull, pblk_dev, in_place ? nullptr : w.JTJ0);
       }
       if (need_mx) {
         if (wt || os_misaligned) {
@@ -1301,6 +1358,87 @@ extern "C" double dirac_b200_normal_eq_weighted(dirac_b200_problem *pr, int clus
     DB_CHECK(cudaMemcpy(JTJ, w.JTJ0, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost));
   DB_CHECK(cudaGetLastError());
   return c;
+}
+
+// ------------------------------------------------------------------------------------------------
+// test hooks of the damped assembly: J^T J + mu I of one (cluster, chunk) at pblk, lower triangle
+// only, for each mu in turn in the same buffer (factor: dpotrf(LOWER) in place after each write, so
+// every later mu rebuilds over the previous factor).  out [nmu][8N][8N], info [nmu] (factor only).
+// ------------------------------------------------------------------------------------------------
+extern "C" void dirac_b200_assemble_damped(dirac_b200_problem *pr, int clus, int chunk,
+                                           const double *pblk, int nmu, const double *mus,
+                                           int factor, double *out, int *info) {
+  DevProblem &d = pr->d;
+  db_lm_init(pr);
+  LMWork &w = pr->lm;
+  const int n = w.n8;
+  int t0, t1;
+  chunk_range(d, clus, chunk, &t0, &t1);
+  DB_CHECK(cudaMemcpyAsync(w.pnew, pblk, sizeof(double) * n, cudaMemcpyHostToDevice, d.stream));
+  gram(pr, clus, t0, t1, 1, w.Tsub);
+  assemble(pr, w.Tsub, w.pnew, nullptr);
+  for (int i = 0; i < nmu; i++) {
+    AssembleArgs a = assemble_args(d, w.Tsub, w.pnew, w.Hst);
+    a.JTJ = w.JTJ;
+    a.mu = mus[i];
+    a.lower = 1;
+    assemble_tiles(pr, a, 1);
+    if (factor)
+      CS_CHECK(cusolverDnDpotrf(w.cs, CUBLAS_FILL_MODE_LOWER, n, w.JTJ, n, w.cswork, w.lwork,
+                                w.devinfo));
+    DB_CHECK(cudaMemcpyAsync(out + (size_t)i * n * n, w.JTJ, sizeof(double) * (size_t)n * n,
+                             cudaMemcpyDeviceToHost, d.stream));
+    if (factor)
+      DB_CHECK(cudaMemcpyAsync(info + i, w.devinfo, sizeof(int), cudaMemcpyDeviceToHost, d.stream));
+    db_stream_sync(d.stream);
+  }
+  DB_CHECK(cudaGetLastError());
+}
+
+// the batched assembly of the sweep's first systems over the local clusters list[0..nb) (first
+// chunk each, Jones from the full vector pp, which replaces the problem's): mu0 = tau max diag -> mu_out [nb]; out [nb][8N][8N]
+// gets J^T J + mu0 I, lower triangle only (lower) or the full undamped matrix
+extern "C" void dirac_b200_assemble_batch(dirac_b200_problem *pr, const double *pp, const int *list,
+                                          int nb, double tau, int lower, double *mu_out, double *out) {
+  DevProblem &d = pr->d;
+  db_lm_init(pr);
+  DB_CHECK(cudaMemcpy(d.pp, pp, sizeof(double) * d.npar, cudaMemcpyHostToDevice));
+  LMWork &w = pr->lm;
+  const size_t nn = (size_t)w.n8 * w.n8;
+  std::vector<int> tix(d.M), poff(d.M);
+  for (int k = 0; k < d.M; k++) {
+    tix[k] = d.h_clus[k].chunk0;
+    poff[k] = d.h_chunk_poff[tix[k]];
+  }
+  for (int y = 0; y < nb; y++) {
+    const int k = list[y];
+    int t0, t1;
+    chunk_range(d, k, 0, &t0, &t1);
+    gram(pr, k, t0, t1, 1, w.T + (size_t)tix[k] * d.Nbase * 16);
+    w.T_valid[tix[k]] = 1;
+  }
+  int *ibuf = dalloc<int>(nb + 2 * d.M);
+  double *H = dalloc<double>((size_t)4 * d.N * nb), *mu = dalloc<double>(nb);
+  double *A = dalloc<double>(nn * nb);
+  DB_CHECK(cudaMemcpy(ibuf, list, sizeof(int) * nb, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(ibuf + nb, tix.data(), sizeof(int) * d.M, cudaMemcpyHostToDevice));
+  DB_CHECK(cudaMemcpy(ibuf + nb + d.M, poff.data(), sizeof(int) * d.M, cudaMemcpyHostToDevice));
+  AssembleArgs b = assemble_args(d, w.T, d.pp, H);
+  b.list = ibuf; b.tix = ibuf + nb; b.poff = ibuf + nb + d.M;
+  b.JTJ = A;
+  b.stride = (long long)nn;
+  station_sums(pr, b, nb);
+  db_launch_batch_mu0(H, mu, d.N, tau, nb, d.stream);
+  if (lower) {
+    b.mu_dev = mu;
+    b.lower = 1;
+  }
+  assemble_tiles(pr, b, nb);
+  DB_CHECK(cudaMemcpyAsync(mu_out, mu, sizeof(double) * nb, cudaMemcpyDeviceToHost, d.stream));
+  DB_CHECK(cudaMemcpyAsync(out, A, sizeof(double) * nn * nb, cudaMemcpyDeviceToHost, d.stream));
+  db_stream_sync(d.stream);
+  db_free(ibuf); db_free(H); db_free(mu); db_free(A);
+  DB_CHECK(cudaGetLastError());
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -44,7 +44,8 @@ struct LMWork {
   double *pold;           // [8N] Jones at the start of the visit (sharded closing pass)
   // normal matrices of ALL clusters of a sweep, assembled and factorised in one batch before the
   // sweep (each cluster's first LM solve then only needs the triangular solves)
-  double *JB, *LB;        // [M][8N][8N] J^T J and its damped Cholesky factor
+  double *JB, *LB;        // [M][8N][8N] J^T J (cluster solvers only, else null) and the damped
+                          // Cholesky factor
   size_t lb_stride;       // doubles between two factors in LB
   int lb_ld, binfo_step;  // leading dimension of a factor; ints per matrix in the status array
   double *HB;             // [M][N][4]
@@ -55,6 +56,10 @@ struct LMWork {
   int *blist_dev, *btix_dev, *bpoff_dev;
   int *pref_slot;         // host [M]: slot of cluster k in the current batch, -1 if not prefactored
   const double *jtj0_cur; // matrix the damping loop of the current iteration starts from
+  // in-place Cholesky of an unweighted system (8N beyond the cluster solver): the Gram tensors, Jones
+  // and station sums the damped solves assemble J^T J + mu I from (sys_T null: the system is in JTJ0
+  // or jtj0_cur and is copied with the damping)
+  const double *sys_T, *sys_p, *sys_H;
 };
 
 struct dirac_b200_problem {
