@@ -10,6 +10,7 @@
 //                       (weighted, robust LM: one streaming pass)              k_weighted_jtj
 //   (J^T J + mu I) dp   linsolv 0: k_chol_solve / k_tri_solve on one thread-block cluster
 //                       (kernels_chol.cu; cuSOLVER potrf/potrs when 8N > 512 or no cluster)
+//                       (8N > 1024: the sweep's first systems by one blocked batch, bigchol.cu)
 //                       linsolv 1, 2: cuSOLVER geqrf+ormqr+trsm | gesvd
 // The dense n x 8N Jacobian of the reference (7.2 GB per cluster at N=62, T=120) never exists.
 #include <float.h>
@@ -123,6 +124,7 @@ void db_lm_init(dirac_b200_problem *pr) {
   w.own_chol = n8 <= db_chol_max_n() && db_chol_available() && !getenv("DIRAC_B200_CUSOLVER");
   if (w.own_chol && (size_t)w.lwork < db_chol_ws_doubles(n8)) w.lwork = (int)db_chol_ws_doubles(n8);
   w.cswork = dalloc<double>((size_t)w.lwork);
+  w.bc = (!w.own_chol && n8 > 1024) ? db_bigchol_create(n8, BC_BLOCK, BC_INV_PANEL, BC_LOOKAHEAD) : nullptr;
   w.bt_ws = nullptr;
   w.bt_epoch = 0;
   if (!w.own_chol && db_bigtri_available(n8)) {
@@ -159,6 +161,7 @@ void db_lm_free(dirac_b200_problem *pr) {
   db_free(w.Hst); db_free(w.pnew); db_free(w.plast); db_free(w.pold); db_free(w.jte_part);
   db_free(w.tau); db_free(w.cswork); db_free(w.dbuf);
   if (w.bt_ws) db_free(w.bt_ws);
+  db_bigchol_destroy(w.bc);
   if (w.svdS) { db_free(w.svdS); db_free(w.svdU); db_free(w.svdVT); }
   if (w.wbuf) { db_free(w.wbuf); db_free(w.ebuf); db_free(w.HP); db_free(w.HQ); }
   if (w.os_eps) { db_free(w.os_eps); db_free(w.os_w); }
@@ -464,6 +467,7 @@ void db_prefactor_sweep(dirac_b200_problem *pr, double tau) {
     DB_CHECK(cudaMemcpy(w.btix_dev, tix.data(), sizeof(int) * d.M, cudaMemcpyHostToDevice));
     DB_CHECK(cudaMemcpy(w.bpoff_dev, poff.data(), sizeof(int) * d.M, cudaMemcpyHostToDevice));
     DB_CHECK(cudaMemcpy(w.LBptr_dev, ptr.data(), sizeof(double *) * d.M, cudaMemcpyHostToDevice));
+    if (w.bc) db_bigchol_bind_batch(w.bc, w.LB, (long long)lstride, d.M);
   }
   std::vector<int> list;
   // Gram tensors still missing: one launch per run of consecutive single-chunk clusters (their slots
@@ -523,46 +527,13 @@ void db_prefactor_sweep(dirac_b200_problem *pr, double tau) {
     db_launch_chol_factor_batched(w.JB, n, w.mu_dev, w.LB, (long long)lstride, w.binfo_dev, nb,
                                   d.stream);
     db_count_launch(1);
-  } else if (n <= 1024) {
+  } else if (!w.bc) {
     CS_CHECK(cusolverDnDpotrfBatched(w.cs, CUBLAS_FILL_MODE_LOWER, n, w.LBptr_dev, n, w.binfo_dev, nb));
     db_count_launch(1);
   } else {
-    // Large systems (8N = 4096 at 512 stations: 23 GFLOP each): the batched routine is a small-matrix
-    // code; a single dpotrf leaves most SMs idle in its panel phases (~10 TFLOP/s).  The clusters'
-    // first systems are independent, so they are factorised side by side on a few streams.
-    enum { NS = 4 };
-    static cudaStream_t fs[NS];
-    static cusolverDnHandle_t fh[NS];
-    static double *fwork[NS];
-    static int flwork = 0;
-    static cudaEvent_t fev[NS], fstart;
-    if (!flwork || flwork < w.lwork) {
-      for (int i = 0; i < NS; i++) {
-        if (!flwork) {
-          DB_CHECK(cudaStreamCreateWithFlags(&fs[i], cudaStreamNonBlocking));
-          CS_CHECK(cusolverDnCreate(&fh[i]));
-          CS_CHECK(cusolverDnSetStream(fh[i], fs[i]));
-          DB_CHECK(cudaEventCreateWithFlags(&fev[i], cudaEventDisableTiming));
-        } else {
-          db_free(fwork[i]);
-        }
-        fwork[i] = dalloc<double>((size_t)w.lwork);
-      }
-      if (!flwork) DB_CHECK(cudaEventCreateWithFlags(&fstart, cudaEventDisableTiming));
-      flwork = w.lwork;
-    }
-    DB_CHECK(cudaEventRecord(fstart, d.stream));
-    for (int i = 0; i < NS && i < nb; i++) DB_CHECK(cudaStreamWaitEvent(fs[i], fstart, 0));
-    for (int b = 0; b < nb; b++) {
-      const int i = b % NS;
-      CS_CHECK(cusolverDnDpotrf(fh[i], CUBLAS_FILL_MODE_LOWER, n, w.LB + nn * b, n, fwork[i], flwork,
-                                w.binfo_dev + b));
-    }
-    for (int i = 0; i < NS && i < nb; i++) {
-      DB_CHECK(cudaEventRecord(fev[i], fs[i]));
-      DB_CHECK(cudaStreamWaitEvent(d.stream, fev[i], 0));
-    }
-    db_count_launch(nb);
+    // Large systems (8N = 4096 at 512 stations: 23 GFLOP each): one blocked panel loop over all of
+    // them (bigchol.cu), its trailing updates DGEMMs over the whole batch
+    db_bigchol_factor_batch(w.bc, nb, w.binfo_dev, 1, d.stream);
   }
   db_prof_end(d.stream);
   DB_CHECK(cudaMemcpyAsync(w.h_mu, w.mu_dev, sizeof(double) * nb, cudaMemcpyDeviceToHost, d.stream));

@@ -8,6 +8,19 @@
 #include "../../include/dirac_b200.h"
 #include "internal.cuh"
 
+// blocked Cholesky of the sweep's batch of large systems (bigchol.cu)
+struct BigChol;
+// panels of nbk columns; inv_panel: the panel solve by the inverse of the diagonal block and a DGEMM;
+// lookahead: panel j+1 on a second stream while the rest of panel j's trailing update runs
+BigChol *db_bigchol_create(int n, int nbk, bool inv_panel, bool lookahead);
+// what the LM runs (measured at n = 4096, 32 systems: DESIGN.md §5.2)
+enum { BC_BLOCK = 256 };
+static const bool BC_INV_PANEL = true, BC_LOOKAHEAD = true;
+void db_bigchol_destroy(BigChol *bc);
+// the batch: system b at A0 + b * stride, b < maxb (uploads the panels' pointer arrays)
+void db_bigchol_bind_batch(BigChol *bc, double *A0, long long stride, int maxb);
+void db_bigchol_factor_batch(BigChol *bc, int nb, int *info, int info_step, cudaStream_t st);
+
 struct LMWork {
   bool ready;
   int n8;                 // 8N
@@ -26,6 +39,7 @@ struct LMWork {
   bool own_chol;  // damped solves by the cluster Cholesky kernel (else cuSOLVER)
   double *bt_ws;  // large systems: workspace of the blocked triangular solves (kernels_bigtri.cu)
   unsigned bt_epoch;
+  BigChol *bc;    // large systems: blocked factorisation of the sweep's batch (bigchol.cu)
   double *jte_part;       // per-CTA station sums of the linear-mapped gradient pass
   bool step_armed, step_fused;  // trial point formed by the solver kernel's epilogue
   double *jtj_spec;       // J^T J assembled speculatively at the trial point (nullptr: none)
