@@ -493,7 +493,9 @@ unsigned long long dirac_b200_launch_count(void);
  * (k_chol_solve / k_tri_solve / batched potrf), 6 k_weighted_jtj, 7 line setup, 8 k_cluster_pass
  * without gradient (ADD / SUB / cost-only; kind 2 then counts the gradient-carrying INIT / TRIAL passes),
  * 9 k_rtr_stats (row condensation of the RTR / NSD solvers), 10 k_rtr_eval, 13 k_stream_band (cost
- * or residual of every channel of a minibatch band), 14 k_grad_tma_band (its gradient).  enable(1) clears the
+ * or residual of every channel of a minibatch band), 14 k_grad_tma_band (its gradient), 15 k_beam_tables
+ * (station beam tables), 16 k_sky_predict<0> of a stochastic interval (coherencies into device
+ * storage).  enable(1) clears the
  * records; read returns the launch count and sums the elapsed
  * milliseconds and the algorithmic bytes of the recorded launches of that kind. */
 unsigned long long dirac_b200_kernel_count(int kind); /* launches of `kind` since load */

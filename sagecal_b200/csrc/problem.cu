@@ -34,13 +34,15 @@ static cudaEvent_t prof_event() {
   DB_CHECK(cudaEventCreate(&e));
   return e;
 }
-// kinds: 13 k_stream_band (band cost or residual), 14 k_grad_tma_band (band gradient)
-static unsigned long long g_kind_count[15] = {0};
+// kinds: 13 k_stream_band (band cost or residual), 14 k_grad_tma_band (band gradient), 15
+// k_beam_tables (station beam tables), 16 the stochastic interval's coherency predictions
+#define DB_PROF_KINDS 17
+static unsigned long long g_kind_count[DB_PROF_KINDS] = {0};
 extern "C" unsigned long long dirac_b200_kernel_count(int kind) {
-  return (kind >= 0 && kind < 15) ? g_kind_count[kind] : 0ull;
+  return (kind >= 0 && kind < DB_PROF_KINDS) ? g_kind_count[kind] : 0ull;
 }
 void db_prof_begin(int kind, double bytes, cudaStream_t st) {
-  if (kind >= 0 && kind < 15) g_kind_count[kind]++;
+  if (kind >= 0 && kind < DB_PROF_KINDS) g_kind_count[kind]++;
   if (!g_prof_on) return;
   ProfRec r; r.a = prof_event(); r.b = prof_event(); r.kind = kind; r.bytes = bytes;
   DB_CHECK(cudaEventRecord(r.a, st));

@@ -498,46 +498,67 @@ class DiracAPI:
             self.lib.bfgsfit_minibatch_consensus(*head, dptr(Y), dptr(Z), dptr(rho), *tail)
         return r0.value, r1.value
 
+    @staticmethod
+    def _interval_fn(L, name, argtypes, beam, nmb, tmb):
+        """the interval call `name`, or its _withbeam variant with the beam arguments inserted after
+        uvmax (the 17th argument) when beam is given; returns (function, beam arguments)"""
+        if beam is None:
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = C.c_int, argtypes
+            return fn, ()
+        assert beam.tilesz == nmb * tmb, "time_utc is [minibatches][tmb]"
+        dpp = C.POINTER(c_double_p)
+        fn = getattr(L, name + "_withbeam")
+        fn.restype = C.c_int
+        fn.argtypes = argtypes[:17] + [C.c_int] + [C.c_double] * 5 + [c_double_p] * 3 + [
+            c_int_p, dpp, dpp, dpp, C.POINTER(elementcoeff), C.c_int] + argtypes[17:]
+        return fn, (*beam.head(), *beam.tail())
+
     def stochastic_interval(self, u, v, w, xo, N, Nbase, tmb, barr, sky: SkyModel, freqs, deltaf, pt,
                             pfreq, nsolbw, nepochs, uvmin=0.0, uvmax=1e9, max_lbfgs=4, lbfgs_m=5,
-                            robust_nu=2.0, ccid=-99999, rho=1e-9, phase_only=0):
+                            robust_nu=2.0, ccid=-99999, rho=1e-9, phase_only=0,
+                            beam: "BeamSetup" = None):
         """dirac_b200_stochastic_interval: the minibatch driver's loop over one interval in one call.
         u, v, w [minibatches, Nbase*tmb]; xo [minibatches, Nchan, Nbase*tmb*8] data -> residual (in
         place); barr: minibatches * Nbase*tmb rows (input only); pt: nsolbw persistent_data_t
         (persist_init_array); pfreq [nsolbw, 8 N Mt] start -> solutions (in
-        place).  returns (retval, res_00, res_01), each [nepochs, minibatches, nsolbw]"""
-        L = self.lib
-        L.dirac_b200_stochastic_interval.restype = C.c_int
-        L.dirac_b200_stochastic_interval.argtypes = [c_double_p] * 4 + [C.c_int] * 4 + [
-            C.POINTER(baseline_t), C.POINTER(clus_source_t), C.c_int, C.c_int, c_double_p, C.c_int,
-            C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double,
-            C.c_void_p, c_double_p, C.c_int, C.c_double, C.c_int, c_double_p, c_double_p]
+        place); beam: station beams through dirac_b200_stochastic_interval_withbeam, its time_utc
+        [minibatches][tmb].  returns (retval, res_00, res_01), each [nepochs, minibatches, nsolbw]"""
         for a in (u, v, w, xo, pfreq):
             assert a.dtype == np.float64 and a.flags.c_contiguous
         freqs = np.ascontiguousarray(freqs, dtype=np.float64)
         nmb = u.shape[0]
+        fn, bargs = self._interval_fn(self.lib, "dirac_b200_stochastic_interval", [c_double_p] * 4 + [
+            C.c_int] * 4 + [
+            C.POINTER(baseline_t), C.POINTER(clus_source_t), C.c_int, C.c_int, c_double_p, C.c_int,
+            C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double,
+            C.c_void_p, c_double_p, C.c_int, C.c_double, C.c_int, c_double_p, c_double_p], beam, nmb,
+            tmb)
         r0 = np.zeros((nepochs, nmb, nsolbw))
         r1 = np.zeros((nepochs, nmb, nsolbw))
-        rv = L.dirac_b200_stochastic_interval(
+        rv = fn(
             dptr(u), dptr(v), dptr(w), dptr(xo), N, Nbase, tmb, nmb, barr, sky.arr, sky.M, sky.Mt,
-            dptr(freqs), len(freqs), deltaf, uvmin, uvmax, nsolbw, nepochs, max_lbfgs, lbfgs_m,
-            robust_nu, C.cast(pt, C.c_void_p), dptr(pfreq), ccid, rho, phase_only, dptr(r0), dptr(r1))
+            dptr(freqs), len(freqs), deltaf, uvmin, uvmax, *bargs, nsolbw, nepochs, max_lbfgs,
+            lbfgs_m, robust_nu, C.cast(pt, C.c_void_p), dptr(pfreq), ccid, rho, phase_only, dptr(r0),
+            dptr(r1))
         return rv, r0, r1
 
     def stochastic_consensus_interval(self, u, v, w, xo, N, Nbase, tmb, barr, sky: SkyModel, freqs,
                                       deltaf, pt, pfreq, nsolbw, nepochs, nadmm, B, Bi, rhok, Z,
                                       use_global=0, uvmin=0.0, uvmax=1e9, max_lbfgs=4, lbfgs_m=5,
-                                      robust_nu=2.0, ccid=-99999, rho=1e-9, phase_only=0):
+                                      robust_nu=2.0, ccid=-99999, rho=1e-9, phase_only=0,
+                                      beam: "BeamSetup" = None):
         """dirac_b200_stochastic_consensus_interval: the consensus minibatch driver's loop over one
         interval in one call.  Arguments as stochastic_interval, plus B [nsolbw, Npoly],
-        Bi [Mt, Npoly, Npoly], rhok [nsolbw, Mt] and Z [Mt, Npoly, 8N] (in place).  returns
+        Bi [Mt, Npoly, Npoly], rhok [nsolbw, Mt] and Z [Mt, Npoly, 8N] (in place); beam: station
+        beams through the _withbeam variant.  returns
         (retval, res_00, res_01 [nadmm, nepochs, minibatches, nsolbw], res_0, res_1, fband [nsolbw])"""
-        L = self.lib
         dp, i, d = c_double_p, C.c_int, C.c_double
-        L.dirac_b200_stochastic_consensus_interval.restype = i
-        L.dirac_b200_stochastic_consensus_interval.argtypes = [dp] * 4 + [i] * 4 + [
+        fn, bargs = self._interval_fn(self.lib, "dirac_b200_stochastic_consensus_interval", [dp] * 4 + [
+            i] * 4 + [
             C.POINTER(baseline_t), C.POINTER(clus_source_t), i, i, dp, i, d, d, d, i, i, i, i, d,
-            C.c_void_p, dp, i, d, i, i, i, dp, dp, dp, dp, i, dp, dp, dp, dp, c_int_p]
+            C.c_void_p, dp, i, d, i, i, i, dp, dp, dp, dp, i, dp, dp, dp, dp, c_int_p], beam,
+            u.shape[0], tmb)
         for a in (u, v, w, xo, pfreq, Z):
             assert a.dtype == np.float64 and a.flags.c_contiguous
         freqs = np.ascontiguousarray(freqs, dtype=np.float64)
@@ -549,9 +570,9 @@ class DiracAPI:
         r01 = np.zeros((nadmm, nepochs, nmb, nsolbw))
         r0, r1 = C.c_double(0.0), C.c_double(0.0)
         fband = np.zeros(max(nsolbw, 1), dtype=np.int32)
-        rv = L.dirac_b200_stochastic_consensus_interval(
+        rv = fn(
             dptr(u), dptr(v), dptr(w), dptr(xo), N, Nbase, tmb, nmb, barr, sky.arr, sky.M, sky.Mt,
-            dptr(freqs), len(freqs), deltaf, uvmin, uvmax, nsolbw, nepochs, max_lbfgs, lbfgs_m,
+            dptr(freqs), len(freqs), deltaf, uvmin, uvmax, *bargs, nsolbw, nepochs, max_lbfgs, lbfgs_m,
             robust_nu, C.cast(pt, C.c_void_p), dptr(pfreq), ccid, rho, phase_only, nadmm, B.shape[1],
             dptr(B), dptr(Bi), dptr(rhok), dptr(Z), use_global, dptr(r00), dptr(r01), C.byref(r0),
             C.byref(r1), fband.ctypes.data_as(c_int_p))

@@ -55,7 +55,8 @@ CHANNELS_EXPORTED = ["calculate_residuals", "dirac_b200_bfgsfit_channels", "dira
 #: every symbol include/dirac_b200_stochastic.h declares (stochastic calibration of an interval, with
 #: or without spectral consensus over the bands)
 STOCHASTIC_EXPORTED = ["dirac_b200_stochastic_interval", "dirac_b200_stochastic_consensus_interval",
-                       "dirac_b200_consensus_bands_update"]
+                       "dirac_b200_consensus_bands_update", "dirac_b200_stochastic_interval_withbeam",
+                       "dirac_b200_stochastic_consensus_interval_withbeam"]
 
 
 class DiracB200(DiracAPI):
