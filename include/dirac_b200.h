@@ -536,4 +536,6 @@ int dirac_b200_bigtri_solve(int n, const double *L, const double *b, double *x, 
 #include "dirac_b200_channels.h"
 /* stochastic calibration of a whole solution interval (the minibatch driver's loop in one call) */
 #include "dirac_b200_stochastic.h"
+/* federated stochastic calibration (the projectback manifold average and the slave's ADMM step) */
+#include "dirac_b200_federated.h"
 #endif

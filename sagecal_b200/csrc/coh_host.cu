@@ -1099,6 +1099,93 @@ extern "C" int dirac_b200_stochastic_consensus_interval_withbeam(
       res_01, res_0, res_1, fband);
 }
 // Dirac_radio.h:666 (residual.c:1620-1740): simulation with solutions
+
+// The federated stochastic slave's interval (sagecal_stochastic_slave.cpp:650-881) for one measurement
+// set on this rank, with the master's exchange (sagecal_stochastic_master.cpp:334-354) done on every
+// rank after one all-reduce.  The coherencies are predicted once; the slave predicts them in every
+// pass with the reloaded flags and the uv cut (:675-723), so every pass here fits the cut rows' flags
+// (DESIGN.md 7 items 24, 25).  Y, X and Zavg start from zero; Z is the caller's.
+extern "C" int dirac_b200_stochastic_federated_interval(
+    double *u, double *v, double *w, double *xo, int N, int Nbase, int tmb, int minibatches,
+    baseline_t *barr, clus_source_t *carr, int M, int Mt, double *freqs, int Nchan, double deltaf,
+    double uvmin, double uvmax, int nsolbw, int nepochs, int max_lbfgs, int lbfgs_m, double robust_nu,
+    persistent_data_t *pt, double *pfreq, int ccid, double rho, int phase_only, int nadmm, int Npoly,
+    double *B, double *Bi, double *rhok, double *alphak, double *Z, int use_global, int randomize,
+    int rank, int world, dirac_b200_allreduce_fn allreduce, void *user, double *res_00,
+    double *res_01, double *res_0, double *res_1, int *fband) {
+  const char *fn = "dirac_b200_stochastic_federated_interval";
+  if (bands_refused(fn, nsolbw, Nchan)) return -1;
+  if (nadmm < 1 || Npoly < 1) {
+    fprintf(stderr, "%s: nadmm = %d ADMM iterations, Npoly = %d polynomial terms; each must be at "
+                    "least 1\n", fn, nadmm, Npoly);
+    return -1;
+  }
+  if (world < 1 || world > 64 || rank < 0 || rank >= world) {
+    fprintf(stderr, "%s: rank %d of world %d; 0 <= rank < world <= 64\n", fn, rank, world);
+    return -1;
+  }
+  if (world > 1 && !allreduce && db_nccl_world() != world) {
+    fprintf(stderr, "%s: world %d without an exchange: give a callback or call dirac_b200_nccl_init "
+                    "with %d ranks first\n", fn, world, world);
+    return -1;
+  }
+  const size_t m = (size_t)8 * N * Mt, L = m * Npoly;
+  DeviceScope ds;
+  IntervalDev iv;
+  interval_stage(ds, iv, u, v, w, xo, N, Nbase, tmb, minibatches, barr, carr, M, freqs, Nchan, deltaf,
+                 uvmin, uvmax, nsolbw, nullptr);
+  std::vector<double> Y((size_t)nsolbw * m, 0.0), z(m), X(L, 0.0), Zavg(L, 0.0), ex((size_t)world * L + Mt);
+  // [world][L] solutions | [Mt] rank 0's draws
+  double *dex = ds.alloc<double>(ex.size());
+  int *dcr = ds.alloc<int>(Mt);
+  std::vector<int> cr(Mt);
+  BandDev *bd = db_band_create(N, Nbase, tmb, carr, M, Mt, iv.nper, ds.st);
+  for (int ad = 0; ad < nadmm; ad++) {
+    for (int ep = 0; ep < nepochs; ep++)
+      for (int mb = 0; mb < minibatches; mb++) {
+        const size_t o = (((size_t)ad * nepochs + ep) * minibatches + mb) * nsolbw;
+        for (int b = 0; b < nsolbw; b++) {
+          db_consensus_bz(Z, B + (size_t)b * Npoly, N, Mt, Npoly, z.data());
+          db_band_fit(bd, iv.band(mb, b, true), pfreq + b * m, Y.data() + b * m, z.data(),
+                      rhok + (size_t)b * Mt, max_lbfgs, lbfgs_m, robust_nu, res_00 + o + b,
+                      res_01 + o + b, pt + b);
+        }
+        dirac_b200_federated_bands_update(N, Mt, nsolbw, Npoly, ad, res_00 + o, res_01 + o, pfreq, B,
+                                          Bi, rhok, alphak, Zavg.data(), X.data(), res_0, res_1,
+                                          Y.data(), Z, fband);
+      }
+    // the exchange (:857-880): gather every rank's Z and rank 0's draws, average on every rank
+    std::fill(ex.begin(), ex.end(), 0.0);
+    std::copy(Z, Z + L, ex.begin() + (size_t)rank * L);
+    if (rank == 0)
+      for (int k = 0; k < Mt; k++) ex[(size_t)world * L + k] = randomize ? (double)(rand() % world) : 0.0;
+    DB_CHECK(cudaMemcpyAsync(dex, ex.data(), sizeof(double) * ex.size(), cudaMemcpyHostToDevice, ds.st));
+    if (world > 1) db_allreduce_stream(allreduce, user, dex, (long long)ex.size(), ds.st);
+    DB_CHECK(cudaMemcpyAsync(ex.data() + (size_t)world * L, dex + (size_t)world * L,
+                             sizeof(double) * Mt, cudaMemcpyDeviceToHost, ds.st));
+    db_stream_sync(ds.st);
+    for (int k = 0; k < Mt; k++) cr[k] = (int)ex[(size_t)world * L + k];
+    DB_CHECK(cudaMemcpyAsync(dcr, cr.data(), sizeof(int) * Mt, cudaMemcpyHostToDevice, ds.st));
+    if (db_manifold_projectback(dex, N * Npoly, Mt, world, ad == 0 ? 10 : 2, dcr, ds.st)) exit(1);
+    DB_CHECK(cudaMemcpyAsync(Zavg.data(), dex + (size_t)rank * L, sizeof(double) * L,
+                             cudaMemcpyDeviceToHost, ds.st));
+    db_stream_sync(ds.st);
+    // X_k += alpha_k (Z_k - Zavg_k)
+    for (int k = 0; k < Mt; k++)
+      for (size_t i = 0; i < (size_t)8 * N * Npoly; i++) {
+        const size_t j = (size_t)k * 8 * N * Npoly + i;
+        X[j] += alphak[k] * (Z[j] - Zavg[j]);
+      }
+  }
+  db_band_destroy(bd);
+  if (use_global)
+    for (int b = 0; b < nsolbw; b++)
+      db_consensus_bz(Z, B + (size_t)b * Npoly, N, Mt, Npoly, pfreq + b * m);
+  interval_residuals(ds, iv, barr, carr, N, M, minibatches, nsolbw, pfreq, m, ccid, rho, phase_only,
+                     xo);
+  return 0;
+}
+
 extern "C" int predict_visibilities_multifreq_withsol(double *u, double *v, double *w, double *p,
                                                       double *x, int *ignorelist, int N, int Nbase,
                                                       int tilesz, baseline_t *barr,

@@ -137,6 +137,27 @@ void db_allreduce_world(dirac_b200_problem *pr, void *dev, long long count) {
   }
 }
 
+// the size of the communicator of dirac_b200_nccl_init (0: none)
+int db_nccl_world() { return g_nccl.comm ? g_nccl.world : 0; }
+
+// sum a device buffer of doubles over the ranks through the host's callback, or the communicator of
+// dirac_b200_nccl_init when there is none; enqueued on st
+void db_allreduce_stream(dirac_b200_allreduce_fn fn, void *user, void *dev, long long count,
+                         cudaStream_t st) {
+  if (count <= 0) return;
+  if (fn) {
+    fn(dev, count, (void *)st, user);
+  } else {
+    if (!g_nccl.comm) {
+      fprintf(stderr, "dirac_b200: an exchange without a callback or a communicator\n");
+      exit(1);
+    }
+    NCCL_CHECK(g_nccl.AllReduce(dev, dev, (size_t)count, DB_NCCL_DOUBLE, DB_NCCL_SUM, g_nccl.comm, st));
+  }
+  g_comm_calls++;
+  g_comm_bytes += (unsigned long long)count * 8ull;
+}
+
 // ---- overlapped exchange: all-reduces on a communication stream of the library, grouped ----------
 // Used where a streaming kernel is followed by a large all-reduce of what it wrote (the LBFGS line
 // model: three visibility-sized vectors per iteration): the kernel is launched in time chunks and

@@ -152,6 +152,33 @@ extern "C" int dirac_b200_consensus_prod_inverse(const double *B, double *Bi, in
   return 0;
 }
 
+// Bi[k] = (sum_f rho[k + f*M] B_f B_f^T + alpha_k I)^-1 as find_prod_inverse_full_fed
+// (consensus_poly.c:381-451, 546-600) forms it: every singular value s > 1e-12 becomes 1/(s + alpha_k),
+// every other one 1/alpha_k (so a singular sum with alpha_k = 0 gives inf, as the reference's does)
+extern "C" int dirac_b200_consensus_prod_inverse_fed(const double *B, double *Bi, int Npoly, int Nf,
+                                                     int M, const double *rho, const double *alpha) {
+  const int n = Npoly;
+  std::vector<double> A((size_t)n * n), V, w;
+  for (int k = 0; k < M; k++) {
+    std::fill(A.begin(), A.end(), 0.0);
+    for (int f = 0; f < Nf; f++) {
+      const double r = rho[k + (size_t)f * M];
+      for (int i = 0; i < n; i++)
+        for (int j = 0; j < n; j++) A[i * n + j] += r * B[f * n + i] * B[f * n + j];
+    }
+    jacobi_eig(A, n, V, w);
+    double *out = Bi + (size_t)k * n * n;
+    for (int i = 0; i < n; i++)
+      for (int j = 0; j < n; j++) {
+        double s = 0.0;
+        for (int e = 0; e < n; e++)
+          s += V[i * n + e] * V[j * n + e] * (w[e] > 1e-12 ? 1.0 / (w[e] + alpha[k]) : 1.0 / alpha[k]);
+        out[i * n + j] = s;
+      }
+  }
+  return 0;
+}
+
 // ---- the ADMM step of the spectral consensus over bands (minibatch_consensus_mode.cpp:524-601) ------
 // z = B_b Z of every chunk, as the driver sums it (:526-531): z[ci] = sum_p Bb[p] Z[ci][p]
 void db_consensus_bz(const double *Z, const double *Bb, int N, int Mt, int Npoly, double *z) {
@@ -219,6 +246,95 @@ extern "C" int dirac_b200_consensus_bands_update(int N, int Mt, int nsolbw, int 
     }
   }
   // Z[ci][p] = sum_q Bi[ci][p][q] z[q][ci], Z laid out [Mt][Npoly][8N]
+  for (int ci = 0; ci < Mt; ci++)
+    for (int p = 0; p < Npoly; p++) {
+      double *Zp = Z + n8 * ((size_t)ci * Npoly + p);
+      const double *bi = Bi + ((size_t)ci * Npoly + p) * Npoly;
+      for (size_t i = 0; i < n8; i++) {
+        double s = 0.0;
+        for (int q = 0; q < Npoly; q++) s += bi[q] * z[(size_t)q * m + n8 * ci + i];
+        Zp[i] = s;
+      }
+    }
+  // Y_b <- Y_b - rho_b B_b Z for the good bands
+  std::vector<double> bz(m);
+  for (int b = 0; b < nsolbw; b++) {
+    if (fband[b]) continue;
+    db_consensus_bz(Z, B + (size_t)b * Npoly, N, Mt, Npoly, bz.data());
+    for (int ci = 0; ci < Mt; ci++) {
+      const double r = rhok[(size_t)b * Mt + ci];
+      double *y = Y + (size_t)b * m + n8 * ci;
+      for (size_t i = 0; i < n8; i++) y[i] += -r * bz[n8 * ci + i];
+    }
+  }
+  return 0;
+}
+
+// The federated slave's step after the bands of one minibatch (sagecal_stochastic_slave.cpp:731-852),
+// decision for decision, with one MS per rank.  Where it differs from the in-process step above
+// (DESIGN.md 7): res_0 / res_1 are the plain mean over the bands of this minibatch; z starts from zero
+// when band 0 is flagged; from ADMM iteration 1 on, z[p][ci] += alpha_k Zavg[ci][p] - X[ci][p].
+extern "C" int dirac_b200_federated_bands_update(int N, int Mt, int nsolbw, int Npoly, int admm,
+                                                 const double *res_00, const double *res_01,
+                                                 const double *pfreq, const double *B,
+                                                 const double *Bi, const double *rhok,
+                                                 const double *alphak, const double *Zavg,
+                                                 const double *X, double *res_0, double *res_1,
+                                                 double *Y, double *Z, int *fband) {
+  if (N < 1 || Mt < 1 || nsolbw < 1 || Npoly < 1 || admm < 0) {
+    fprintf(stderr, "dirac_b200_federated_bands_update: N = %d, Mt = %d, nsolbw = %d, Npoly = %d "
+                    "must be at least 1 and admm = %d at least 0\n", N, Mt, nsolbw, Npoly, admm);
+    return -1;
+  }
+  const size_t n8 = (size_t)8 * N, m = n8 * Mt;
+  const double res_ratio = 1.5, clm_dbl_max = 1e12;  // sagecal_stochastic_slave.cpp res_ratio, CLM_DBL_MAX
+  std::vector<double> resband(nsolbw);
+  double r0 = 0.0, r1 = 0.0;
+  for (int b = 0; b < nsolbw; b++) {
+    r0 += res_00[b];
+    r1 += res_01[b];
+    resband[b] = res_00[b] > 0.0 && res_01[b] > 0.0 ? res_01[b] : clm_dbl_max;
+  }
+  r0 /= (double)nsolbw;
+  r1 /= (double)nsolbw;
+  *res_0 = r0;
+  *res_1 = r1;
+  for (int b = 0; b < nsolbw; b++) fband[b] = resband[b] > res_ratio * r1 ? 1 : 0;
+  // Y_b <- Y_b + rho_b J_b for the good bands
+  for (int b = 0; b < nsolbw; b++) {
+    if (fband[b]) continue;
+    for (int ci = 0; ci < Mt; ci++) {
+      const double r = rhok[(size_t)b * Mt + ci];
+      const double *J = pfreq + (size_t)b * m + n8 * ci;
+      double *y = Y + (size_t)b * m + n8 * ci;
+      for (size_t i = 0; i < n8; i++) y[i] += r * J[i];
+    }
+  }
+  // z[p] = sum over the good bands of B_b[p] Y_b, laid out [Npoly][Mt][8N] (:783-797)
+  std::vector<double> z((size_t)Npoly * m, 0.0);
+  if (!fband[0])
+    for (int p = 0; p < Npoly; p++)
+      for (size_t i = 0; i < m; i++) z[(size_t)p * m + i] = B[p] * Y[i];
+  for (int b = 1; b < nsolbw; b++) {
+    if (fband[b]) continue;
+    for (int p = 0; p < Npoly; p++) {
+      const double bp = B[(size_t)b * Npoly + p];
+      const double *y = Y + (size_t)b * m;
+      double *zp = z.data() + (size_t)p * m;
+      for (size_t i = 0; i < m; i++) zp[i] += bp * y[i];
+    }
+  }
+  // the federated-averaging term, Zavg and X laid out [Mt][Npoly][8N] like Z (:805-826)
+  if (admm > 0)
+    for (int ci = 0; ci < Mt; ci++)
+      for (int p = 0; p < Npoly; p++) {
+        const double *za = Zavg + n8 * ((size_t)ci * Npoly + p);
+        const double *x = X + n8 * ((size_t)ci * Npoly + p);
+        double *zp = z.data() + (size_t)p * m + n8 * ci;
+        for (size_t i = 0; i < n8; i++) zp[i] += alphak[ci] * za[i];
+        for (size_t i = 0; i < n8; i++) zp[i] += -x[i];
+      }
+  // Z[ci][p] = sum_q Bi[ci][p][q] z[q][ci]
   for (int ci = 0; ci < Mt; ci++)
     for (int p = 0; p < Npoly; p++) {
       double *Zp = Z + n8 * ((size_t)ci * Npoly + p);

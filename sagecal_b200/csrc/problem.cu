@@ -35,8 +35,9 @@ static cudaEvent_t prof_event() {
   return e;
 }
 // kinds: 13 k_stream_band (band cost or residual), 14 k_grad_tma_band (band gradient), 15
-// k_beam_tables (station beam tables), 16 the stochastic interval's coherency predictions
-#define DB_PROF_KINDS 17
+// k_beam_tables (station beam tables), 16 the stochastic interval's coherency predictions, 17
+// k_manifold_projectback
+#define DB_PROF_KINDS 18
 static unsigned long long g_kind_count[DB_PROF_KINDS] = {0};
 extern "C" unsigned long long dirac_b200_kernel_count(int kind) {
   return (kind >= 0 && kind < DB_PROF_KINDS) ? g_kind_count[kind] : 0ull;

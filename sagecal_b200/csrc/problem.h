@@ -179,7 +179,12 @@ void db_allreduce(dirac_b200_problem *pr, void *dev, long long count);
 // sum over the ranks of the process-wide communicator regardless of cluster sharding (consensus over
 // subbands: every rank holds its own, unsharded problem); no-op without a communicator
 void db_allreduce_world(dirac_b200_problem *pr, void *dev, long long count);
-void db_lm_set_aug(const double *y_dev, const double *bz_dev, const double *y_host,
+int db_nccl_world();
+void db_allreduce_stream(dirac_b200_allreduce_fn fn, void *user, void *dev, long long count,
+                         cudaStream_t st);
+// the projectback manifold average on device memory (kernels_manifold.cu)
+int db_manifold_projectback(double *Y, int n, int Mt, int Nf, int Niter, const int *cr,
+                            cudaStream_t st);void db_lm_set_aug(const double *y_dev, const double *bz_dev, const double *y_host,
                    const double *bz_host, double rho);
 int db_overlap_available(const dirac_b200_problem *pr);
 cudaStream_t db_comm_stream();

@@ -578,6 +578,40 @@ class DiracAPI:
             C.byref(r1), fband.ctypes.data_as(c_int_p))
         return rv, r00, r01, r0.value, r1.value, fband[:nsolbw]
 
+    def stochastic_federated_interval(self, u, v, w, xo, N, Nbase, tmb, barr, sky: SkyModel, freqs,
+                                      deltaf, pt, pfreq, nsolbw, nepochs, nadmm, B, Bi, rhok, alphak,
+                                      Z, use_global=0, randomize=0, rank=0, world=1, allreduce=None,
+                                      uvmin=0.0, uvmax=1e9, max_lbfgs=4, lbfgs_m=5, robust_nu=2.0,
+                                      ccid=-99999, rho=1e-9, phase_only=0):
+        """dirac_b200_stochastic_federated_interval: the federated slave's interval on this rank in one
+        call.  Arguments as stochastic_consensus_interval, plus alphak [Mt], randomize, rank, world and
+        allreduce (a ctypes callback of sagecal_b200.dist.make_allreduce, or None for the library's NCCL
+        communicator).  returns
+        (retval, res_00, res_01 [nadmm, nepochs, minibatches, nsolbw], res_0, res_1, fband [nsolbw])"""
+        dp, i, d = c_double_p, C.c_int, C.c_double
+        fn = self.lib.dirac_b200_stochastic_federated_interval
+        fn.restype = i
+        fn.argtypes = ([dp] * 4 + [i] * 4 + [C.POINTER(baseline_t), C.POINTER(clus_source_t), i, i, dp, i,
+                       d, d, d, i, i, i, i, d, C.c_void_p, dp, i, d, i, i, i, dp, dp, dp, dp, dp, i, i,
+                       i, i, C.c_void_p, C.c_void_p, dp, dp, dp, dp, c_int_p])
+        for a in (u, v, w, xo, pfreq, Z):
+            assert a.dtype == np.float64 and a.flags.c_contiguous
+        freqs, B, Bi, rhok, alphak = [np.ascontiguousarray(a, dtype=np.float64)
+                                      for a in (freqs, B, Bi, rhok, alphak)]
+        nmb = u.shape[0]
+        r00 = np.zeros((nadmm, nepochs, nmb, nsolbw))
+        r01 = np.zeros((nadmm, nepochs, nmb, nsolbw))
+        r0, r1 = C.c_double(0.0), C.c_double(0.0)
+        fband = np.zeros(max(nsolbw, 1), dtype=np.int32)
+        cb = C.cast(allreduce, C.c_void_p) if allreduce is not None else None
+        rv = fn(dptr(u), dptr(v), dptr(w), dptr(xo), N, Nbase, tmb, nmb, barr, sky.arr, sky.M, sky.Mt,
+                dptr(freqs), len(freqs), deltaf, uvmin, uvmax, nsolbw, nepochs, max_lbfgs, lbfgs_m,
+                robust_nu, C.cast(pt, C.c_void_p), dptr(pfreq), ccid, rho, phase_only, nadmm, B.shape[1],
+                dptr(B), dptr(Bi), dptr(rhok), dptr(alphak), dptr(Z), use_global, randomize, rank,
+                world, cb, None, dptr(r00), dptr(r01), C.byref(r0), C.byref(r1),
+                fband.ctypes.data_as(c_int_p))
+        return rv, r00, r01, r0.value, r1.value, fband[:nsolbw]
+
     def consensus_bands_update(self, N, res_00, res_01, pfreq, B, Bi, rhok, res_0, res_1, Y, Z):
         """dirac_b200_consensus_bands_update: the ADMM step after the bands of one minibatch.
         pfreq, Y [nsolbw, 8 N Mt]; B [nsolbw, Npoly]; Bi [Mt, Npoly, Npoly]; rhok [nsolbw, Mt];
@@ -597,6 +631,76 @@ class DiracAPI:
         r0, r1 = C.c_double(res_0), C.c_double(res_1)
         fband = np.zeros(max(nsolbw, 1), dtype=np.int32)
         rv = L.dirac_b200_consensus_bands_update(N, Mt, nsolbw, Npoly, dptr(r00), dptr(r01),
+                                                 *[dptr(a) for a in args], C.byref(r0), C.byref(r1),
+                                                 dptr(Y), dptr(Z), fband.ctypes.data_as(c_int_p))
+        return rv, r0.value, r1.value, fband[:nsolbw]
+
+    def manifold_projectback(self, Y, Niter, randomize=0):
+        """calculate_manifold_average_projectback on Y [Nf, M, 8N] in place (Nt is not used);
+        returns the status"""
+        L = self.lib
+        L.calculate_manifold_average_projectback.restype = C.c_int
+        L.calculate_manifold_average_projectback.argtypes = [C.c_int] * 3 + [c_double_p] + [C.c_int] * 3
+        assert Y.dtype == np.float64 and Y.flags.c_contiguous and Y.ndim == 3
+        Nf, M, n8 = Y.shape
+        return L.calculate_manifold_average_projectback(n8 // 8, M, Nf, dptr(Y), Niter, randomize, 1)
+
+    def manifold_projectback_dev(self, Y, Niter, cr=None, stream=None):
+        """dirac_b200_manifold_projectback_dev on a CUDA float64 tensor Y [Nf, M, 8N] in place, on the
+        given stream (a torch.cuda.Stream; default: torch's current stream); cr [M] host ints or None"""
+        import torch
+        L = self.lib
+        L.dirac_b200_manifold_projectback_dev.restype = C.c_int
+        L.dirac_b200_manifold_projectback_dev.argtypes = ([C.c_int] * 3 + [C.c_void_p, C.c_int, c_int_p,
+                                                           C.c_void_p])
+        assert Y.is_cuda and Y.dtype == torch.float64 and Y.is_contiguous() and Y.dim() == 3
+        Nf, M, n8 = Y.shape
+        st = (stream or torch.cuda.current_stream(Y.device)).cuda_stream
+        crp = None
+        if cr is not None:
+            cr = np.ascontiguousarray(cr, dtype=np.int32)
+            crp = cr.ctypes.data_as(c_int_p)
+        return L.dirac_b200_manifold_projectback_dev(n8 // 8, M, Nf, C.c_void_p(Y.data_ptr()), Niter,
+                                                      crp, C.c_void_p(st))
+
+    def consensus_prod_inverse_fed(self, B, rho, alpha):
+        """dirac_b200_consensus_prod_inverse_fed: B [Nf, Npoly], rho [Nf, M], alpha [M];
+        returns Bi [M, Npoly, Npoly]"""
+        L = self.lib
+        dp = c_double_p
+        L.dirac_b200_consensus_prod_inverse_fed.restype = C.c_int
+        L.dirac_b200_consensus_prod_inverse_fed.argtypes = [dp, dp, C.c_int, C.c_int, C.c_int, dp, dp]
+        Nf, Npoly = B.shape
+        M = rho.shape[1]
+        B = np.ascontiguousarray(B, dtype=np.float64)
+        rho = np.ascontiguousarray(rho, dtype=np.float64)
+        alpha = np.ascontiguousarray(alpha, dtype=np.float64)
+        Bi = np.zeros((M, Npoly, Npoly))
+        rv = L.dirac_b200_consensus_prod_inverse_fed(dptr(B), dptr(Bi), Npoly, Nf, M, dptr(rho),
+                                                     dptr(alpha))
+        assert rv == 0
+        return Bi
+
+    def federated_bands_update(self, N, admm, res_00, res_01, pfreq, B, Bi, rhok, alphak, Zavg, X,
+                               Y, Z):
+        """dirac_b200_federated_bands_update: the federated slave's ADMM step after the bands of one
+        minibatch.  Shapes as consensus_bands_update; alphak [Mt]; Zavg, X [Mt, Npoly, 8N].  Y and Z
+        in place; returns (retval, res_0, res_1, fband)"""
+        L = self.lib
+        dp = c_double_p
+        L.dirac_b200_federated_bands_update.restype = C.c_int
+        L.dirac_b200_federated_bands_update.argtypes = [C.c_int] * 5 + [dp] * 9 + [dp, dp, dp, dp,
+                                                                                 c_int_p]
+        nsolbw, Npoly = B.shape
+        Mt = Bi.shape[0]
+        for a in (Y, Z):
+            assert a.dtype == np.float64 and a.flags.c_contiguous
+        r00 = np.ascontiguousarray(res_00, dtype=np.float64)
+        r01 = np.ascontiguousarray(res_01, dtype=np.float64)
+        args = [np.ascontiguousarray(a, dtype=np.float64) for a in (pfreq, B, Bi, rhok, alphak, Zavg, X)]
+        r0, r1 = C.c_double(0.0), C.c_double(0.0)
+        fband = np.zeros(max(nsolbw, 1), dtype=np.int32)
+        rv = L.dirac_b200_federated_bands_update(N, Mt, nsolbw, Npoly, admm, dptr(r00), dptr(r01),
                                                  *[dptr(a) for a in args], C.byref(r0), C.byref(r1),
                                                  dptr(Y), dptr(Z), fband.ctypes.data_as(c_int_p))
         return rv, r0.value, r1.value, fband[:nsolbw]

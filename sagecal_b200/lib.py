@@ -58,6 +58,10 @@ STOCHASTIC_EXPORTED = ["dirac_b200_stochastic_interval", "dirac_b200_stochastic_
                        "dirac_b200_consensus_bands_update", "dirac_b200_stochastic_interval_withbeam",
                        "dirac_b200_stochastic_consensus_interval_withbeam"]
 
+#: every symbol include/dirac_b200_federated.h declares (federated stochastic calibration)
+FEDERATED_EXPORTED = ["dirac_b200_stochastic_federated_interval", "calculate_manifold_average_projectback", "dirac_b200_manifold_projectback_dev",
+                      "dirac_b200_consensus_prod_inverse_fed", "dirac_b200_federated_bands_update"]
+
 
 class DiracB200(DiracAPI):
     """The product library: the reference entry points (inherited bindings) plus the thin
