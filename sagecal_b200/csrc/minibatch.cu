@@ -264,45 +264,89 @@ void db_lbfgs_fit_minibatch(dirac_b200_problem *pr, double *p, int m, int itmax,
 }
 
 // the reference's host arrays as one band: channel c's coherencies coh[c][row][M][4] (complex) and data
-// x[c][row][8] (robust_batchmode_lbfgs.c:1176-1183) go up once, into the planar band layout
+// x[c][row][8] (robust_batchmode_lbfgs.c:1176-1183) go up once, into the planar band layout, with the
+// flags of barr's rows; the buffers live as long as ds
+static BandView band_stage(DeviceScope &ds, const double *x, int N, int Nbase, int tilesz,
+                           const baseline_t *barr, const double *coh, int M, int Nf) {
+  const long long R = (long long)Nbase * tilesz;
+  std::vector<unsigned char> hflag(R);
+  db_canonical_flags(N, Nbase, tilesz, barr, hflag.data());
+  const int nc = Nf > 0 ? Nf : 0;
+  double2 *dcoh = ds.alloc<double2>((size_t)M * 4 * R * (nc ? nc : 1));
+  double2 *dx = ds.alloc<double2>((size_t)4 * R * (nc ? nc : 1));
+  unsigned char *dflag = ds.upload(hflag);
+  long long rows_per = (128ll << 20) / ((long long)M * 64);
+  if (rows_per < 1) rows_per = 1;
+  if (rows_per > R) rows_per = R;
+  // stages rows_per rows of one channel's coherencies, or one channel's data
+  const size_t nstage = (size_t)rows_per * M * 4 > (size_t)4 * R ? (size_t)rows_per * M * 4 : 4 * R;
+  double2 *stage = ds.alloc<double2>(nstage);
+  for (int c = 0; c < nc; c++) {
+    double2 *cc = dcoh + (size_t)c * M * 4 * R;
+    for (long long r0 = 0; r0 < R; r0 += rows_per) {
+      const int nr = (int)((R - r0 < rows_per) ? (R - r0) : rows_per);
+      DB_CHECK(cudaMemcpyAsync(stage, coh + ((size_t)c * R + r0) * M * 8, (size_t)nr * M * 64,
+                               cudaMemcpyHostToDevice, ds.st));
+      db_launch_coh_to_planar(stage, cc, r0, nr, M, R, ds.st);
+      db_count_launch(1);
+    }
+    db_count_coh_host_bytes((size_t)R * M * 64);
+    DB_CHECK(cudaMemcpyAsync(stage, x + (size_t)c * 8 * R, (size_t)R * 64, cudaMemcpyHostToDevice,
+                             ds.st));
+    db_launch_vis_to_planar(stage, dx + (size_t)c * 4 * R, R, ds.st);
+    db_count_launch(1);
+  }
+  BandView b = {dcoh, dx, dflag, nc};
+  return b;
+}
+
 static int minibatch_fit(double *x, int N, int Nbase, int tilesz, baseline_t *barr,
                          clus_source_t *carr, double *coh, int M, int Mt, int Nf, double *p,
                          const double *y, const double *z, const double *rho, int max_lbfgs,
                          int lbfgs_m, double robust_nu, double *res_0, double *res_1,
                          persistent_data_t *indata) {
-  const long long R = (long long)Nbase * tilesz;
-  std::vector<unsigned char> hflag(R);
-  db_canonical_flags(N, Nbase, tilesz, barr, hflag.data());
   {
     DeviceScope ds;
     BandDev *bd = db_band_create(N, Nbase, tilesz, carr, M, Mt, Nf, ds.st);
-    const int nc = Nf > 0 ? Nf : 0;
-    double2 *dcoh = ds.alloc<double2>((size_t)M * 4 * R * (nc ? nc : 1));
-    double2 *dx = ds.alloc<double2>((size_t)4 * R * (nc ? nc : 1));
-    unsigned char *dflag = ds.upload(hflag);
-    long long rows_per = (128ll << 20) / ((long long)M * 64);
-    if (rows_per < 1) rows_per = 1;
-    if (rows_per > R) rows_per = R;
-    // stages rows_per rows of one channel's coherencies, or one channel's data
-    const size_t nstage = (size_t)rows_per * M * 4 > (size_t)4 * R ? (size_t)rows_per * M * 4 : 4 * R;
-    double2 *stage = ds.alloc<double2>(nstage);
-    for (int c = 0; c < nc; c++) {
-      double2 *cc = dcoh + (size_t)c * M * 4 * R;
-      for (long long r0 = 0; r0 < R; r0 += rows_per) {
-        const int nr = (int)((R - r0 < rows_per) ? (R - r0) : rows_per);
-        DB_CHECK(cudaMemcpyAsync(stage, coh + ((size_t)c * R + r0) * M * 8, (size_t)nr * M * 64,
-                                 cudaMemcpyHostToDevice, ds.st));
-        db_launch_coh_to_planar(stage, cc, r0, nr, M, R, ds.st);
-        db_count_launch(1);
-      }
-      db_count_coh_host_bytes((size_t)R * M * 64);
-      DB_CHECK(cudaMemcpyAsync(stage, x + (size_t)c * 8 * R, (size_t)R * 64, cudaMemcpyHostToDevice,
-                               ds.st));
-      db_launch_vis_to_planar(stage, dx + (size_t)c * 4 * R, R, ds.st);
-      db_count_launch(1);
-    }
-    BandView b = {dcoh, dx, dflag, nc};
+    const BandView b = band_stage(ds, x, N, Nbase, tilesz, barr, coh, M, Nf);
     db_band_fit(bd, b, p, y, z, rho, max_lbfgs, lbfgs_m, robust_nu, res_0, res_1, indata);
+    db_band_destroy(bd);
+    ds.sync();
+  }
+  return 0;
+}
+
+// Test hook (not in the public headers): the band passes the minibatch fits run, on one band staged
+// as minibatch_fit stages it, in a BandDev of capacity maxnc >= Nf.  The npts Jones vectors p[i]
+// (8 N Mt each) are evaluated in order with the fits' own cost and gradient: cost[i] the Student's-t
+// cost summed over the channels (plus the consensus terms when y, z, rho are given), grad[i] its
+// gradient with the reference's minibatch sign; res [Nf][R][8] (or null) the residual x - V of the
+// last point's gradient pass.  Returns -1 for Nf < 0, Nf > maxnc or npts < 1, before any device work.
+extern "C" int dirac_b200_band_eval(int N, int Nbase, int tilesz, baseline_t *barr, clus_source_t *carr,
+                                    int M, int Mt, const double *coh, const double *x, int Nf,
+                                    int maxnc, int npts, const double *p, const double *y,
+                                    const double *z, const double *rho, double nu, double *cost,
+                                    double *grad, double *res) {
+  if (Nf < 0 || Nf > maxnc || npts < 1) return -1;
+  {
+    DeviceScope ds;
+    BandDev *bd = db_band_create(N, Nbase, tilesz, carr, M, Mt, maxnc, ds.st);
+    const BandView b = band_stage(ds, x, N, Nbase, tilesz, barr, coh, M, Nf);
+    BandFn F = {bd, b, nu, y, z, rho};
+    const size_t m = (size_t)bd->npar;
+    for (int i = 0; i < npts; i++) {
+      cost[i] = F.cost(p + i * m);
+      F.grad(p + i * m, grad + i * m);
+    }
+    if (res && Nf > 0) {
+      double2 *stage = ds.alloc<double2>((size_t)4 * bd->R);
+      for (int c = 0; c < Nf; c++) {
+        db_launch_vis_from_planar(bd->res + (size_t)c * 4 * bd->R, stage, bd->R, ds.st);
+        db_count_launch(1);
+        DB_CHECK(cudaMemcpyAsync(res + (size_t)c * 8 * bd->R, stage, (size_t)bd->R * 64,
+                                 cudaMemcpyDeviceToHost, ds.st));
+      }
+    }
     db_band_destroy(bd);
     ds.sync();
   }

@@ -178,6 +178,37 @@ class DiracB200(DiracAPI):
         g = np.ascontiguousarray(g, dtype=np.float64)
         return float(L.dirac_b200_lbfgs_nrm2(len(g), dptr(g)))
 
+    def band_eval(self, N, Nbase, tilesz, barr, sky: SkyModel, coh, x, Nf, P, nu, maxnc=None,
+                  Y=None, Z=None, rho=None):
+        """the minibatch band passes (dirac_b200_band_eval): one band of Nf channels, coh
+        [Nf][row][M][4] complex and x [Nf][row][8], staged as bfgsfit_minibatch_visibilities stages
+        it, in a band state of capacity maxnc (default Nf); the Jones vectors P [npts, 8 N Mt]
+        evaluated in order with the fits' cost and gradient (consensus terms with Y, Z, rho).
+        returns dict(cost [npts], grad [npts, 8 N Mt], res [Nf * row * 8]: residual of the last
+        point), or None where the hook refuses the arguments"""
+        L = self.lib
+        L.dirac_b200_band_eval.restype = C.c_int
+        L.dirac_b200_band_eval.argtypes = ([C.c_int] * 3 + [C.POINTER(baseline_t),
+                                           C.POINTER(clus_source_t)] + [C.c_int] * 2
+                                           + [c_double_p] * 2 + [C.c_int] * 3 + [c_double_p] * 4
+                                           + [C.c_double] + [c_double_p] * 3)
+        P = np.ascontiguousarray(np.atleast_2d(P), dtype=np.float64)
+        coh = np.ascontiguousarray(coh, dtype=np.complex128)
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        cons = [None if v is None else np.ascontiguousarray(v, dtype=np.float64) for v in (Y, Z, rho)]
+        npts = P.shape[0]
+        cost = np.zeros(max(npts, 1))
+        grad = np.zeros((max(npts, 1), P.shape[1]))
+        res = np.zeros(8 * Nbase * tilesz * max(Nf, 1))
+        rv = L.dirac_b200_band_eval(N, Nbase, tilesz, barr, sky.arr, sky.M, sky.Mt,
+                                    cptr(coh), dptr(x), Nf,
+                                    Nf if maxnc is None else maxnc, npts, dptr(P),
+                                    *[dptr(v) if v is not None else None for v in cons], nu,
+                                    dptr(cost), dptr(grad.reshape(-1)), dptr(res))
+        if rv != 0:
+            return None
+        return dict(cost=cost, grad=grad, res=res[:8 * Nbase * tilesz * Nf])
+
     def kernel_count(self, kind) -> int:
         return int(self.lib.dirac_b200_kernel_count(kind))
 

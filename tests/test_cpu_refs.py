@@ -1,12 +1,15 @@
 """CPU: the plain references the GPU tests of the line model, the RTR evaluator, the IRLS update, the
-LBFGS two-loop recursion and the segmented sky staging lean on, pinned against the restatement
-(oracle/liboracle.so) before a GPU is involved."""
+LBFGS two-loop recursion, the segmented sky staging and the minibatch band passes lean on, pinned
+against the restatement (oracle/liboracle.so) or the compiled reference's recorded answers before a GPU
+is involved."""
 import numpy as np
 import pytest
 
 import orcdirac
-from util import (big_cluster_sky, irls_ref, lbfgs_pairs, line_model_ref, mult_hessian_ref, relerr,
-                  rtr_eval_ref, rtr_weights_ref, small_problem, split_cluster)
+from util import (BAND_CASES, BAND_FAULTS, U64, band_case, band_consensus, band_ref,
+                  big_cluster_sky, irls_ref, lbfgs_pairs, line_model_ref, maps_agree,
+                  mult_hessian_ref, relerr, rtr_eval_ref, rtr_weights_ref, small_problem,
+                  split_cluster)
 
 needs_oracle = pytest.mark.skipif(not orcdirac.available(), reason="oracle/liboracle.so not built")
 
@@ -171,3 +174,120 @@ def test_mult_hessian_reference_matches_oracle(M):
                                                                 np.max(np.abs(got - want) / scale))
         # the pairs matter: the answer is far from the scaled gradient of a memoryless step
         assert relerr(g * (s[0] @ y[0]) / (y[0] @ y[0]), got) > 1e-3
+
+
+# ---- the minibatch band passes: util.band_ref pinned to the compiled reference ----------------------
+def _band_ref_inputs(case):
+    from sagecal_b200.dirac_api import SkyModel, make_barr
+    pr = case["pr"]
+    return make_barr(pr.sta1, pr.sta2, pr.flag), SkyModel(pr.clusters, pr.N)
+
+
+def _ref_band_cost(ref, case, p, nu, cons):
+    """bfgsfit_minibatch_visibilities / _consensus with max_lbfgs = 0: res_0 8 R Nf is
+    robust_cost_func_multifreq at p"""
+    pr = case["pr"]
+    barr, sky = _band_ref_inputs(case)
+    n = 8 * pr.Nbase1 * case["nc"]
+    pt = ref.persist_init(1, case["m"], n, 5)
+    Y, Z, rho = cons if cons is not None else (None, None, None)
+    r0, _ = ref.bfgsfit_minibatch(pr.u, pr.v, pr.w, case["x"].reshape(-1).copy(), pr.N, pr.Nbase,
+                                  pr.tilesz, barr, sky, case["coh"].reshape(-1).copy(), p.copy(),
+                                  case["freqs"], pt, max_lbfgs=0, lbfgs_m=5, robust_nu=nu, Y=Y,
+                                  Z=Z, rho=rho)
+    ref.persist_clear(pt)
+    return r0 * n
+
+
+@pytest.mark.parametrize("consensus", [False, True], ids=["plain", "consensus"])
+@pytest.mark.parametrize("nu", [2.0, 30.0])
+@pytest.mark.parametrize("name", ["n2c3", "n9", "n33h4"])
+def test_band_reference_matches_compiled_reference(ref, name, nu, consensus):
+    """util.band_ref against the compiled reference on bands with non-zero data on flagged and uv-cut
+    rows and hybrid clusters whose row and timeslot chunk maps disagree (n9, n33h4): the cost is
+    robust_cost_func_multifreq (res_0 of a fit with no iterations), the gradient minus the sum over
+    the channels of the single-channel Student's-t gradient (robust_grad_func, which
+    test_gpu_kernels.py pins the full-batch kernel to)"""
+    case = band_case(name)
+    pr = case["pr"]
+    cons = band_consensus(case) if consensus else None
+    barr, sky = _band_ref_inputs(case)
+    R, M = pr.Nbase1, case["M"]
+    worst = 0.0
+    for p in (case["A"], case["B"]):
+        r = band_ref(case, p, nu, *(cons or ()))
+        c_ref = _ref_band_cost(ref, case, p, nu, cons)
+        # res_0 = f * (1/n) and back: two more roundings
+        bound = r["cost_bound"] + 4 * U64 * abs(r["cost"])
+        assert abs(c_ref - r["cost"]) <= bound, (c_ref, r["cost"], bound)
+        worst = max(worst, abs(c_ref - r["cost"]) / bound)
+        g = np.zeros(case["m"])
+        for c in range(case["nc"]):
+            md = ref.me_data(pr.N, pr.Nbase, pr.tilesz, barr, sky,
+                             np.ascontiguousarray(case["coh"][c].reshape(-1)), robust_nu=nu)
+            g -= ref.grad(p.copy(), np.ascontiguousarray(case["x"][c].reshape(-1)), md, robust=True)
+        if cons is not None:
+            y, z, rho = cons
+            g += -y - np.repeat(rho, 8 * pr.N) * (p - z)
+        err = np.abs(g - r["grad"])
+        ratio = err / np.maximum(r["grad_bound"], 1e-300)
+        assert (err <= r["grad_bound"]).all(), ratio.max()
+        worst = max(worst, ratio.max())
+        assert np.abs(r["grad"]).max() > 1e3 * r["grad_bound"].max()
+    print("band_ref vs compiled reference (%s, nu %g): largest error / bound %.3g" % (name, nu, worst))
+
+
+def _dcost(case, p, d, nu, h):
+    """fourth-order central difference of band_ref's cost along d"""
+    f = [band_ref(case, p + t * h * d, nu)["cost"] for t in (-2, -1, 1, 2)]
+    return (f[0] - 8 * f[1] + 8 * f[2] - f[3]) / (12 * h)
+
+
+@pytest.mark.parametrize("name", ["n33h3", "n9"])
+def test_band_reference_gradient_is_minus_the_derivative_of_its_cost(name):
+    """calculus, no other code: on a band whose hybrid chunks are the same under the cost's row map
+    and the gradient's timeslot map (n33h3), d/dt cost(p + t d) = -grad . d along directions confined
+    to each chunk block.  Where the maps disagree (n9: nchunk 2 over 5 timeslots), the reference's
+    gradient is NOT the derivative of its cost, and neither is band_ref's: the rows of timeslot 2
+    that the row map gives to chunk 1 count with chunk 0's Jones"""
+    case = band_case(name)
+    agree = maps_agree(case["tilesz"], case["Nbase"], case["nchunk"])
+    assert agree == (name == "n33h3")
+    N, nu = case["N"], 5.0
+    rng = np.random.default_rng(3)
+    p = case["B"]
+    r = band_ref(case, p, nu)
+    worst_off = 0.0
+    for ci in range(case["Mt"]):
+        d = np.zeros(case["m"])
+        d[8 * N * ci:8 * N * (ci + 1)] = rng.normal(0, 1, 8 * N)
+        fd = _dcost(case, p, d, nu, 1e-4)
+        want = -np.dot(r["grad"], d)
+        scale = np.dot(np.abs(r["grad"]) + r["grad_bound"], np.abs(d))
+        off = abs(fd - want) / scale
+        worst_off = max(worst_off, off)
+        if agree:
+            assert off < 1e-8, (ci, fd, want)
+    if not agree:
+        assert worst_off > 1e-3, worst_off
+
+
+def test_band_cases_discriminate():
+    """every deliberate fault of BAND_FAULTS, applied to band_ref, moves some quantity of some GPU case
+    (test_gpu_band.py) past its bound by more than 10^3: the case set can see it"""
+    names = [n for n in BAND_CASES if n != "n62"]   # the smaller cases already reach every fault
+    cases = [band_case(n) for n in names]
+    for fault in BAND_FAULTS:
+        worst = 0.0
+        for case in cases:
+            for p in (case["A"], case["B"]):
+                for nu in (2.0, 30.0):
+                    good = band_ref(case, p, nu)
+                    bad = band_ref(case, p, nu, fault=fault)
+                    worst = max(worst,
+                                abs(bad["cost"] - good["cost"]) / good["cost_bound"],
+                                (np.abs(bad["res"] - good["res"]) / good["res_bound"]).max(),
+                                (np.abs(bad["grad"] - good["grad"])
+                                 / np.maximum(good["grad_bound"], 1e-300)).max())
+        print("fault %s: largest error / bound %.3g" % (fault, worst))
+        assert worst > 1e3, (fault, worst)

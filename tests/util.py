@@ -564,3 +564,227 @@ def lbfgs_start(pr, seed):
     """the perturbed starting Jones of an LBFGS_TRACE_CASES run on the problem of that seed"""
     rng = np.random.default_rng(seed + 100)
     return pr.pp0 + 0.1 * rng.normal(0, 1, pr.pp0.shape)
+
+
+# ---- the minibatch band passes (k_stream_band, k_grad_tma_band) ------------------------------------------
+U64 = 2.0 ** -53   # unit roundoff of float64
+
+#: (N, M, timeslots, channels, nchunk of the clusters, capacity maxnc) of the band cases
+BAND_CASES = {
+    "n2c1": (2, 1, 1, 1, [1], 1),
+    "n2c3": (2, 1, 1, 3, [1], 3),
+    "n9": (9, 3, 5, 2, [1, 2, 1], 2),
+    "n33h3": (33, 7, 9, 5, [1, 3, 1, 1, 3, 1, 1], 5),
+    "n33h4": (33, 7, 9, 5, [1, 4, 1, 1, 4, 1, 1], 5),
+    "n62": (62, 64, 11, 4, [2 if k % 8 == 3 else (3 if k == 60 else 1) for k in range(64)], 4),
+    "n9c33": (9, 2, 2, 33, [1, 1], 40),
+    "n9all": (9, 3, 5, 2, [1, 2, 1], 2),
+}
+
+
+def maps_agree(tilesz, Nbase, nchunk):
+    """whether the cost's row map (chunk_index over the rows) and the gradient's timeslot map
+    (timeslot / ceil(tilesz / nchunk)) put every row in the same chunk"""
+    R = Nbase * tilesz
+    rows = np.arange(R)
+    return all(np.array_equal(synth.chunk_index(rows, R, n), (rows // Nbase) // (-(-tilesz // n)))
+               for n in nchunk)
+
+
+def band_case(name, seed=41):
+    """one band of a minibatch: a problem of BAND_CASES[name] observed at nc frequencies with the same
+    Jones, data with noise and outliers and NON-ZERO on flagged rows; random flag-1 and uv-cut
+    (flag 2) rows, one station and one timeslot fully flagged where others remain ("n9all": every
+    row flagged).  Jones points: A near the truth (small residuals), B far from it (large).
+    returns a dict: the problem fields, coh [nc][row][M][4] complex, x [nc][row][8], A, B, maxnc"""
+    N, M, T, nc, nchunk, maxnc = BAND_CASES[name]
+    rng = np.random.default_rng(seed + 7 * N + T)
+    pr = synth.make_problem(N=N, M=M, tilesz=T, seed=seed + N, kmean=1.0, nchunk=nchunk,
+                            flag_frac=0.0, uvcut_frac=0.0, with_data=False)
+    R, Nb = pr.Nbase1, pr.Nbase
+    fl = np.zeros(R, dtype=np.uint8)
+    u = rng.uniform(0, 1, R)
+    fl[u < 0.06] = 1
+    fl[(u >= 0.06) & (u < 0.1)] = 2
+    if N > 2:
+        s = N // 2
+        fl[(pr.sta1 == s) | (pr.sta2 == s)] = 1
+    if T > 1:
+        fl[:Nb] = 2
+    if name == "n9all":
+        fl[:] = 1
+    pr.flag = fl
+    freqs = 140e6 + 4e6 * np.arange(nc)
+    cohs, xs = [], []
+    for f in freqs:
+        coh = synth.coherencies(pr.u, pr.v, pr.w, pr.clusters, f, pr.fdelta)
+        x = synth.apply_jones(coh, pr.jones_true, pr.sta1, pr.sta2, N, pr.nchunk)
+        sig = 1e-3 * np.median(np.abs(x))
+        x = x + rng.normal(0, sig, x.shape)
+        bad = rng.uniform(0, 1, x.shape) < 0.01
+        x[bad] += rng.normal(0, 50 * sig, int(bad.sum()))
+        cohs.append(coh.reshape(R, M, 4))
+        xs.append(x.reshape(R, 8))
+    m = 8 * N * pr.Mt
+    A = pr.jones_true + 1e-4 * rng.normal(0, 1, m)
+    B = pr.jones_true + 0.3 * rng.normal(0, 1, m)
+    return dict(pr=pr, name=name, N=N, Nbase=Nb, tilesz=T, M=M, Mt=pr.Mt, nc=nc, nchunk=pr.nchunk,
+                sta1=pr.sta1, sta2=pr.sta2, flag=fl, freqs=freqs, coh=np.array(cohs), x=np.array(xs),
+                A=A, B=B, maxnc=maxnc, m=m)
+
+
+def band_consensus(case, seed=5):
+    """consensus terms (y, z, rho) of a band case"""
+    rng = np.random.default_rng(seed)
+    m = case["m"]
+    return (0.1 * rng.normal(0, 1, m), case["pr"].jones_true + 0.05 * rng.normal(0, 1, m),
+            rng.uniform(1.0, 10.0, case["Mt"]))
+
+
+#: deliberate faults band_ref can apply to itself (tests/test_cpu_refs.py: sensitivity of the cases)
+BAND_FAULTS = ("cost_timeslot_map", "grad_row_map", "drop_flagged_cost", "channel0_coherencies",
+               "drop_last_timeslot_block", "drop_last_baseline_group", "grad_sign")
+
+
+def _mm2(A, B):
+    """products of stacks of 2x2 matrices, written out (broadcast over the leading axes)"""
+    out = np.empty(np.broadcast_shapes(A.shape, B.shape), dtype=np.result_type(A, B))
+    for i in range(2):
+        for j in range(2):
+            out[..., i, j] = A[..., i, 0] * B[..., 0, j] + A[..., i, 1] * B[..., 1, j]
+    return out
+
+
+def _scatter2(idx, V, n):
+    """sum of the 2x2 matrices V [rows, 2, 2] into n slots by idx [rows]"""
+    out = np.zeros((n, 2, 2), dtype=V.dtype)
+    for i in range(2):
+        for j in range(2):
+            v = V[:, i, j]
+            if np.iscomplexobj(v):
+                out[:, i, j] = (np.bincount(idx, v.real, n) + 1j * np.bincount(idx, v.imag, n))
+            else:
+                out[:, i, j] = np.bincount(idx, v, n)
+    return out
+
+
+def band_ref(case, p, nu, y=None, z=None, rho=None, fault=None):
+    """plain per-row float64 restatement of one band's minibatch passes
+    (robust_cost_func_multifreq / robust_grad_func_multifreq, robust_batchmode_lbfgs.c:1096-1440):
+      model     V = sum_k Jp C_k Jq^H, chunk of the row by the row map (chunk_index), zero on every
+                flagged row (flag 1 and uv-cut 2)
+      residual  e = x - V [nc][row][8]
+      cost      sum log(1.0 + e e (1/nu)) over every channel, row and real component (func_robust_th)
+      gradient  minus the sum over channels of the full-batch Student's-t gradient: 2 sum psi(e) dV/dtheta,
+                psi(e) = e / (nu + e^2), over the unflagged rows, chunk by the timeslot map
+                (timeslot / ceil(tilesz / nchunk), :1186-1196)
+      consensus cost + sum_ci y.(p - z) + rho_ci/2 |p - z|^2, gradient - y - rho_ci (p - z)
+    with the a-priori error budgets of any evaluation of the same sums in float64:
+      res_bound  (M + 10) u (|x| + sum_k |Jp||C_k||Jq|^T) per element
+      cost_bound rounding of each term, the residual error through 2e/(nu + e^2), the summation
+      grad_bound per component: the rounding of 2 sum |psi(e)||dV/dtheta| plus the residual error
+                 through psi'(e)
+    The reference sum is accumulated in long double (lsum).  `fault` (one of BAND_FAULTS) makes the
+    restatement deliberately wrong.  returns dict(cost, res, grad, res_bound, cost_bound, grad_bound)"""
+    N, Nb, T, M, nc = case["N"], case["Nbase"], case["tilesz"], case["M"], case["nc"]
+    R = Nb * T
+    u = U64
+    sta1, sta2 = case["sta1"], case["sta2"]
+    flagged = case["flag"] != 0
+    rows = np.arange(R)
+    tslot = rows // Nb
+    # rows a faulty kernel would never visit (TB = 2 timeslots per block, 32 baselines per group)
+    skip = np.zeros(R, dtype=bool)
+    if fault == "drop_last_timeslot_block":
+        skip = tslot >= ((T - 1) // 2) * 2
+    elif fault == "drop_last_baseline_group":
+        skip = (rows % Nb) >= ((Nb - 1) // 32) * 32
+    coh = np.moveaxis(case["coh"].reshape(nc, R, M, 2, 2), 2, 0)
+    if fault == "channel0_coherencies":
+        coh = np.broadcast_to(coh[:, :1], coh.shape)
+    coh = np.ascontiguousarray(coh)   # [M][nc][row][2][2]
+    xc = case["x"].reshape(nc, R, 4, 2)
+    xc = (xc[..., 0] + 1j * xc[..., 1]).reshape(nc, R, 2, 2)
+    P = np.asarray(p, dtype=np.float64).reshape(-1, N, 4, 2)
+    J = (P[..., 0] + 1j * P[..., 1]).reshape(-1, N, 2, 2)
+    aJ = np.abs(J)
+    H = lambda X: np.conj(np.swapaxes(X, -1, -2))
+    Tt = lambda X: np.swapaxes(X, -1, -2)
+    c0 = np.concatenate([[0], np.cumsum(case["nchunk"])[:-1]]).astype(int)
+    rmaps, tmaps = [], []
+    for k in range(M):
+        nch = case["nchunk"][k]
+        rmaps.append(synth.chunk_index(rows, R, nch))
+        tmaps.append(tslot // (-(-T // nch)))
+    V = np.zeros((nc, R, 2, 2), dtype=np.complex128)
+    Va = np.zeros((nc, R, 2, 2))
+    for k in range(M):
+        cm = c0[k] + (tmaps[k] if fault == "cost_timeslot_map" else rmaps[k])
+        Jp, Jq = J[cm, sta1], J[cm, sta2]
+        V += _mm2(_mm2(Jp, coh[k]), H(Jq))
+        Va += _mm2(_mm2(aJ[cm, sta1], np.abs(coh[k])), Tt(aJ[cm, sta2]))
+    V[:, flagged] = 0.0
+    Va[:, flagged] = 0.0
+    e = xc - V
+    e[:, skip] = 0.0
+    scale = np.abs(xc) + Va
+    res = _api_layout(e.reshape(-1, 2, 2))
+    res_bound = (M + 10) * u * np.repeat(scale.reshape(-1), 2)
+
+    e8 = res.reshape(nc, R, 8)
+    de8 = res_bound.reshape(nc, R, 8)
+    terms = np.log(1.0 + e8 * e8 * (1.0 / nu))
+    keep = ~skip
+    if fault == "drop_flagged_cost":
+        keep = keep & ~flagged
+    terms = terms[:, keep]
+    cost = lsum(terms)
+    nterm = terms.size
+    cost_bound = (lsum(2 * u * (3.0 + np.abs(terms))) + nterm * u * lsum(np.abs(terms))
+                  + lsum((2 * np.abs(e8) / (nu + e8 * e8) * de8)[:, keep]))
+
+    # gradient: per-row weights psi(e) and their error from the residual's, unflagged rows only
+    use = ~flagged & ~skip
+    psi = e8 / (nu + e8 * e8)
+    dpsi = np.abs((nu - e8 * e8) / (nu + e8 * e8) ** 2) * de8
+    W = (psi[..., 0::2] + 1j * psi[..., 1::2]).reshape(nc, R, 2, 2)
+    Wa = (np.abs(psi[..., 0::2]) + np.abs(psi[..., 1::2])).reshape(nc, R, 2, 2)
+    Wd = (dpsi[..., 0::2] + dpsi[..., 1::2]).reshape(nc, R, 2, 2)
+    W[:, ~use] = 0.0
+    Wa[:, ~use] = 0.0
+    Wd[:, ~use] = 0.0
+    Mt = J.shape[0]
+    G = np.zeros((Mt * N, 2, 2), dtype=np.complex128)
+    Ga = np.zeros((Mt * N, 2, 2))
+    Gd = np.zeros((Mt * N, 2, 2))
+    for k in range(M):
+        gm = c0[k] + (rmaps[k] if fault == "grad_row_map" else tmaps[k])
+        C = coh[k]
+        Ca = np.abs(C)
+        Jp, Jq, ap, aq = J[gm, sta1], J[gm, sta2], aJ[gm, sta1], aJ[gm, sta2]
+        ip, iq = gm * N + sta1, gm * N + sta2
+        # d/dJp of Re tr(W^H Jp C Jq^H): W Jq C^H;  d/dJq: W^H Jp C  (real and imaginary parts)
+        n = Mt * N
+        G += _scatter2(ip, _mm2(_mm2(W, Jq), H(C)).sum(axis=0), n)
+        G += _scatter2(iq, _mm2(_mm2(H(W), Jp), C).sum(axis=0), n)
+        Ga += _scatter2(ip, _mm2(_mm2(Wa, aq), Tt(Ca)).sum(axis=0), n)
+        Ga += _scatter2(iq, _mm2(_mm2(Tt(Wa), ap), Ca).sum(axis=0), n)
+        Gd += _scatter2(ip, _mm2(_mm2(Wd, aq), Tt(Ca)).sum(axis=0), n)
+        Gd += _scatter2(iq, _mm2(_mm2(Tt(Wd), ap), Ca).sum(axis=0), n)
+    grad = 2.0 * _api_layout(G.reshape(-1, 2, 2))
+    if fault == "grad_sign":
+        grad = -grad
+    nsum = 8 * nc * max(N - 1, 1) * T + 16
+    grad_bound = np.repeat((2.0 * (nsum * u * Ga + Gd)).reshape(-1), 2)
+
+    if y is not None:
+        d = np.asarray(p) - z
+        rr = np.repeat(np.asarray(rho, dtype=np.float64), 8 * N)
+        cons = y * d + 0.5 * rr * d * d
+        cost = cost + lsum(cons)
+        cost_bound += (len(d) + 4) * u * lsum(np.abs(y * d) + 0.5 * rr * d * d)
+        gc = -y - rr * d
+        grad_bound = grad_bound + 2 * u * (np.abs(grad) + np.abs(y) + rr * np.abs(d))
+        grad = grad + gc
+    return dict(cost=cost, res=res, grad=grad, res_bound=res_bound, cost_bound=cost_bound,
+                grad_bound=grad_bound)
