@@ -252,9 +252,8 @@ struct ClusterPassArgs {
              // 2: ADD   out = in + m          (no cost / jte)
              // 3: SUB   out = in - m          (no cost / jte)
   int write_out;
-  double beta;               // SAGE hidden-data weight: INIT d = beta*in + m ; SUB out = d - m + (1-beta)*in2
-  const double2 *in2;        // mode 3 with beta != 1: the residual the hidden data was formed from
-  const double *pblk_old;    // mode 3 with beta != 1, instead of in2: the Jones the hidden data was
+  double beta;               // SAGE hidden-data weight: INIT d = beta*in + m ; SUB out = d - m + (1-beta)*r_old
+  const double *pblk_old;    // mode 3 with beta != 1: the Jones the hidden data was
                              // formed with; the old residual is recovered as (d - f(p_old))/beta, so
                              // out = d - f(p) + (1-beta)/beta (d - f(p_old)) costs no extra traffic
   int form_hidden;           // modes 1 and 3: `in` is the residual r and the hidden data is formed per
@@ -362,7 +361,9 @@ void db_launch_grad_window_tma(const GradArgs *a, int ntile, long long r_lo, lon
 // every channel of a band: a holds the first channel's coh / res, the grid's z axis the channels
 void db_launch_grad_band_tma(const GradArgs *a, int ntile, int nchan, cudaStream_t st);
 int db_cluster_pass_nblocks(int ntile, int nt, int tslice);
-void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st);
+// the kernel db_launch_cluster_pass launched (DB_CP_NONE: db_cluster_pass had no timeslot to visit)
+enum { DB_CP_LIN = 0, DB_CP_LIN_GRAD = 1, DB_CP_SPLIT = 2, DB_CP_TILE = 3, DB_CP_NONE = 4 };
+int db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st);
 // whether plain (unweighted) passes of this array take k_cluster_pass_lin, the one variant that
 // forms the hidden data itself (ClusterPassArgs::form_hidden)
 int db_cluster_pass_forms_hidden(int N, int Nbase);

@@ -170,9 +170,10 @@ k_axpby(const double2 *__restrict__ x, double2 *__restrict__ y, long long n4, do
 // hybrid chunk of a row is the ROW-based map px = row / ceil(R/nchunk) of mylm_fit_single_pth
 // (lmfit.c:86): the hidden-data add / subtract of lmfit.c:890-891,980-981 when nchunk does not divide
 // tilesz, i.e. when that map differs from the timeslot ranges the per-chunk LM fits run over.
+// in2 and out may be the same vector (the sharded subtract updates r in place): neither is __restrict__.
 __global__ void __launch_bounds__(256)
 k_cluster_rowmap(const double2 *__restrict__ coh_k, const double2 *__restrict__ in,
-                 const double2 *__restrict__ in2, double2 *__restrict__ out,
+                 const double2 *in2, double2 *out,
                  const unsigned char *__restrict__ flag, const double *__restrict__ pp,
                  const int *__restrict__ chunk_poff, int nchunk, const short2 *__restrict__ blpq,
                  long long R, int Nbase, int sign, double beta) {

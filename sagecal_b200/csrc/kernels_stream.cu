@@ -403,10 +403,12 @@ k_cluster_pass(ClusterPassArgs a) {
           e[c] = csub(d, m[c]);
         }
       } else if (a.mode == 2) {
+        if (a.write_out) {
 #pragma unroll
-        for (int c = 0; c < 4; c++)
-          st_stream(a.out + (long long)c * a.R + row,
-                    cadd(make_double2(a.beta * v[c].x, a.beta * v[c].y), m[c]));
+          for (int c = 0; c < 4; c++)
+            st_stream(a.out + (long long)c * a.R + row,
+                      cadd(make_double2(a.beta * v[c].x, a.beta * v[c].y), m[c]));
+        }
       } else {
         double2 mo[4];
         if (recover) {
@@ -426,10 +428,6 @@ k_cluster_pass(ClusterPassArgs a) {
             // + (1-beta) r_old with r_old = (d - f(p_old)) / beta
             o.x = fma(gamma, v[c].x - mo[c].x, o.x);
             o.y = fma(gamma, v[c].y - mo[c].y, o.y);
-          } else if (a.mode == 3 && a.in2) {
-            const double2 r2 = a.in2[(long long)c * a.R + row];  // may alias out: plain load
-            o.x = fma(1.0 - a.beta, r2.x, o.x);
-            o.y = fma(1.0 - a.beta, r2.y, o.y);
           }
           if (a.write_out) st_stream(a.out + (long long)c * a.R + row, o);
         }
@@ -1010,10 +1008,10 @@ void db_launch_vis_from_planar(const double2 *src, double2 *dst, long long R, cu
 
 int db_cluster_pass_nblocks(int ntile, int nt, int tslice) { return ntile * ((nt + tslice - 1) / tslice); }
 int db_cluster_pass_forms_hidden(int N, int Nbase) { return cluster_pass_lin_fits(N, Nbase); }
-void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st) {
+int db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st) {
   int nt = a->t_end - a->t_begin;
   dim3 grid(ntile, (nt + a->tslice - 1) / a->tslice);
-  if (a->form_hidden && (a->wt || a->in2 || !db_cluster_pass_forms_hidden(a->N, a->Nbase))) {
+  if (a->form_hidden && (a->wt || !db_cluster_pass_forms_hidden(a->N, a->Nbase))) {
     fprintf(stderr, "dirac_b200: cluster pass that forms the hidden data requested where only the tile "
                     "kernels run (%s:%d)\n", __FILE__, __LINE__);
     exit(1);
@@ -1021,14 +1019,19 @@ void db_launch_cluster_pass(const ClusterPassArgs *a, int ntile, cudaStream_t st
   const bool fits = cluster_pass_lin_fits(a->N, a->Nbase);
   if (a->jte == nullptr || (a->mode > 1 && a->mode != 4)) {
     // ADD / SUB / cost-only pass: the linear mapping without the station sums, unless robust
-    // weights or a second input vector ask for the tile kernel
-    if (!a->wt && !a->in2 && fits) launch_cluster_pass_lin<false>(a, st);
-    else k_cluster_pass<<<grid, TILE_THREADS, 0, st>>>(*a);
+    // weights ask for the tile kernel
+    if (!a->wt && fits) {
+      launch_cluster_pass_lin<false>(a, st);
+      return DB_CP_LIN;
+    }
+    k_cluster_pass<<<grid, TILE_THREADS, 0, st>>>(*a);
+    return DB_CP_TILE;
   } else if (a->mode == 4 || a->wt || !fits) {
     k_cluster_pass_split<<<grid, 2 * TILE_THREADS, 0, st>>>(*a);
-  } else {
-    launch_cluster_pass_lin<true>(a, st);
+    return DB_CP_SPLIT;
   }
+  launch_cluster_pass_lin<true>(a, st);
+  return DB_CP_LIN_GRAD;
 }
 void db_launch_coh_gram(const GramArgs *a, int ntile, int nk, cudaStream_t st) {
   dim3 grid(ntile, nk);

@@ -191,23 +191,23 @@ static int pick_tslice(const DevProblem &d, int nt) {
   return ts;
 }
 
-void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
-                     double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
-                     int t1, const double2 *wt, double beta = 1.0, const double2 *in2 = nullptr,
-                     bool jte_zeroed = false, const double *pblk_old = nullptr,
-                     bool form_hidden = false);
+int db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
+                    double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
+                    int t1, const double2 *wt, double beta = 1.0, bool jte_zeroed = false,
+                    const double *pblk_old = nullptr, bool form_hidden = false);
 
-// one streaming pass of cluster k over timeslots [t0,t1): see ClusterPassArgs for the modes
-void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
-                     double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
-                     int t1, const double2 *wt, double beta, const double2 *in2, bool jte_zeroed,
-                     const double *pblk_old, bool form_hidden) {
+// one streaming pass of cluster k over timeslots [t0,t1): see ClusterPassArgs for the modes.
+// Returns the kernel it launched (DB_CP_*; callers other than the test hook ignore it).
+int db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
+                    double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
+                    int t1, const double2 *wt, double beta, bool jte_zeroed,
+                    const double *pblk_old, bool form_hidden) {
   DevProblem &d = pr->d;
   if (t1 <= t0) {
     if (mode <= 1 || mode == 4)
       DB_CHECK(cudaMemsetAsync(d.scal + cost_slot, 0, sizeof(double), d.stream));
     if (jte_dev) DB_CHECK(cudaMemsetAsync(jte_dev, 0, sizeof(double) * 8 * d.N, d.stream));
-    return;
+    return DB_CP_NONE;
   }
   ClusterPassArgs a;
   a.coh_k = d.coh + (size_t)k * 4 * d.R;
@@ -215,7 +215,7 @@ void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, cons
   a.blpq = d.blpq; a.jte_part = pr->lm.jte_part; a.gcounter = d.counters + 16;
   a.partials = pr->partials; a.cost = d.scal + cost_slot; a.counter = d.counters; a.R = d.R;
   a.N = d.N; a.Nbase = d.Nbase; a.t_begin = t0; a.t_end = t1; a.tslice = pick_tslice(d, t1 - t0);
-  a.mode = mode; a.write_out = write_out; a.wt = wt; a.beta = beta; a.in2 = in2;
+  a.mode = mode; a.write_out = write_out; a.wt = wt; a.beta = beta;
   a.pblk_old = pblk_old; a.form_hidden = form_hidden;
   // passes without the gradient accumulator fit two CTAs per SM: twice as many, half as long
   if (!(jte_dev && (mode <= 1 || mode == 4)) && a.tslice > 1)
@@ -225,9 +225,10 @@ void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, cons
   // kind 2: gradient-carrying passes (INIT, TRIAL); kind 8: ADD / SUB / cost-only passes
   db_prof_begin((jte_dev && (mode <= 1 || mode == 4)) ? 2 : 8, (double)(t1 - t0) * d.Nbase * (129.0 + (write_out ? 64.0 : 0.0) +
                                                  (wt ? 64.0 : 0.0)), d.stream);
-  db_launch_cluster_pass(&a, d.ntile, d.stream);
+  const int kernel = db_launch_cluster_pass(&a, d.ntile, d.stream);
   db_prof_end(d.stream);
   db_count_launch(1);
+  return kernel;
 }
 
 // Gram tensor of cluster k over timeslots t0, t0+step, ... < t1 into Tdst [Nbase][16]
@@ -920,11 +921,11 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
           // its residual is the one the visit leaves behind
           const bool last = kiter == itmax - 1;
           db_cluster_pass(pr, k, w.pnew, hidden_from, last ? w.dbuf : nullptr, 1, last ? 1 : 0,
-                          last ? nullptr : w.JTe_new, 1, t0, t1, nullptr, 1.0, nullptr, true, w.pold,
+                          last ? nullptr : w.JTe_new, 1, t0, t1, nullptr, 1.0, true, w.pold,
                           true);
         } else {
           db_cluster_pass(pr, k, w.pnew, w.dbuf, nullptr, 1, 0, os ? nullptr : w.JTe_new, 1, t0, t1,
-                          wt, 1.0, nullptr, true);
+                          wt, 1.0, true);
         }
         if (aug)
           db_launch_lm_aug_rhs(w.JTe_new, w.pnew, aug->y_dev, aug->bz_dev, aug->rho, n, d.stream);
@@ -1130,10 +1131,10 @@ void db_lm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, double
     pr->res = w.dbuf;
     w.dbuf = r;
   } else if (form) {
-    db_cluster_pass(pr, k, pblk_dev, r, r, 3, 1, nullptr, 1, t0, t1, nullptr, 1.0, nullptr, false,
+    db_cluster_pass(pr, k, pblk_dev, r, r, 3, 1, nullptr, 1, t0, t1, nullptr, 1.0, false,
                     w.pold, true);
   } else {
-    db_cluster_pass(pr, k, pblk_dev, w.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta, nullptr,
+    db_cluster_pass(pr, k, pblk_dev, w.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta,
                     false, beta != 1.0 ? w.pold : nullptr);
   }
   fill_info(info, o);
@@ -1144,16 +1145,15 @@ void db_lm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, double
 // (mylm_fit_single_pth, lmfit.c:86,890,980) while the LM fits of its chunks run over the timeslot
 // ranges [ck*ceil(tilesz/nchunk), ...) (lmfit.c:893-905); near the boundaries the hidden data then
 // carries another chunk's Jones.  sign > 0: w.dbuf = beta r + f_k(pp); sign < 0: r = w.dbuf - f_k(pp)
-// (+ (1-beta) r when sharded).
+// (+ (1-beta) r when beta != 1, i.e. when sharded).
 bool db_cluster_needs_rowmap(const dirac_b200_problem *pr, int k) {
   const int nchunk = pr->d.h_clus[k].nchunk;
   return nchunk > 1 && (pr->d.tilesz % nchunk) != 0;
 }
-void db_cluster_hidden(dirac_b200_problem *pr, int k, double2 *r, int sign) {
+void db_cluster_hidden(dirac_b200_problem *pr, int k, double2 *r, int sign, double beta) {
   DevProblem &d = pr->d;
   db_lm_init(pr);
   LMWork &w = pr->lm;
-  const double beta = pr->world > 1 ? pr->beta : 1.0;
   const double2 *coh_k = d.coh + (size_t)k * 4 * d.R;
   const int *poff = d.chunk_poff + d.h_clus[k].chunk0;
   if (sign > 0)
@@ -1276,7 +1276,7 @@ void db_rlm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
   *robust_nu = nu_t;
   // residual of the chunk with the final Jones: r = d - f(p) (+ (1-beta) r when sharded)
   if (!hidden_ready)
-    db_cluster_pass(pr, k, pblk_dev, w.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta, nullptr, false,
+    db_cluster_pass(pr, k, pblk_dev, w.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta, false,
                     beta != 1.0 ? w.pold : nullptr);
   (void)n8;
   fill_info(info, o);
@@ -1487,6 +1487,86 @@ extern "C" void dirac_b200_lm_chunk(dirac_b200_problem *pr, int clus, int chunk,
                            d.stream));
   db_stream_sync(d.stream);
   DB_CHECK(cudaGetLastError());
+}
+
+// One streaming pass of chunk `chunk` of cluster clus through db_cluster_pass, as the LM visits make it:
+// mode 0-4 (ClusterPassArgs), output written or not, J^T e or not, the hidden data formed per row from
+// `in` and pblk_old (form_hidden), hidden-data weight beta.  pblk, pblk_old (or null): 8N Jones; in,
+// wt (or null) and out_init: API layout, full interval.  The device output vector holds out_init
+// before the pass, or is the input vector itself (inplace).  out gets that vector after the pass (all
+// rows), jte [8N] J^T e (0 without), cost the slot the mode writes (slot 2 for mode 0, 1 for modes 1
+// and 4; 0 for ADD / SUB, which have none).  Returns the kernel launched (DB_CP_*), or -1 before any
+// device work for a bad cluster, chunk or mode, mode 4 without J^T e, ADD / SUB with it, form_hidden
+// outside modes 1 and 3, with weights or where the linear-mapped kernel does not run, and a missing
+// pblk_old where form_hidden or a SUB with beta != 1 needs it.
+extern "C" int dirac_b200_cluster_pass_eval(dirac_b200_problem *pr, int clus, int chunk, int mode,
+                                            int write_out, int with_jte, int form_hidden, double beta,
+                                            const double *pblk, const double *pblk_old,
+                                            const double *in, const double *wt,
+                                            const double *out_init, int inplace, double *out,
+                                            double *jte, double *cost) {
+  DevProblem &d = pr->d;
+  if (clus < 0 || clus >= d.M || chunk < 0 || chunk >= d.h_clus[clus].nchunk) return -1;
+  if (mode < 0 || mode > 4 || (mode == 4 && !with_jte) || ((mode == 2 || mode == 3) && with_jte))
+    return -1;
+  if (form_hidden &&
+      ((mode != 1 && mode != 3) || wt || !db_cluster_pass_forms_hidden(d.N, d.Nbase)))
+    return -1;
+  if (!pblk_old && (form_hidden || (mode == 3 && beta != 1.0))) return -1;
+  db_lm_init(pr);
+  LMWork &w = pr->lm;
+  const int n = w.n8;
+  int t0, t1;
+  chunk_range(d, clus, chunk, &t0, &t1);
+  double2 *vin = dalloc<double2>((size_t)4 * d.R);
+  double2 *vout = inplace ? vin : dalloc<double2>((size_t)4 * d.R);
+  double2 *vwt = wt ? dalloc<double2>((size_t)4 * d.R) : nullptr;
+  double *pb = dalloc<double>((size_t)2 * n);
+  db_upload_vis(pr, in, vin);
+  if (!inplace) db_upload_vis(pr, out_init, vout);
+  if (wt) db_upload_vis(pr, wt, vwt);
+  DB_CHECK(cudaMemcpyAsync(pb, pblk, sizeof(double) * n, cudaMemcpyHostToDevice, d.stream));
+  if (pblk_old)
+    DB_CHECK(cudaMemcpyAsync(pb + n, pblk_old, sizeof(double) * n, cudaMemcpyHostToDevice, d.stream));
+  const int slot = mode == 0 ? 2 : 1;
+  const int kernel = db_cluster_pass(pr, clus, pb, vin, vout, mode, write_out,
+                                     with_jte ? w.JTe : nullptr, slot, t0, t1, vwt, beta, false,
+                                     pblk_old ? pb + n : nullptr, form_hidden != 0);
+  db_download_vis(pr, vout, out);
+  if (with_jte)
+    DB_CHECK(cudaMemcpy(jte, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToHost));
+  else
+    memset(jte, 0, sizeof(double) * n);
+  *cost = (mode <= 1 || mode == 4) ? db_read_scalar(pr, slot) : 0.0;
+  db_free(vin);
+  if (!inplace) db_free(vout);
+  db_free(vwt);
+  db_free(pb);
+  DB_CHECK(cudaGetLastError());
+  return kernel;
+}
+
+// db_cluster_hidden: the row-mapped add (sign > 0) or subtract (sign < 0) of cluster clus's model at
+// the full Jones vector pp (it replaces the problem's), with hidden-data weight beta, on the residual
+// r and the hidden data dh (API layout, full interval).  out gets what the call writes: the hidden
+// data (sign > 0) or the residual (sign < 0).  Returns -1 for a bad cluster or sign 0 before any
+// device work.
+extern "C" int dirac_b200_cluster_hidden_eval(dirac_b200_problem *pr, int clus, int sign, double beta,
+                                              const double *pp, const double *r, const double *dh,
+                                              double *out) {
+  DevProblem &d = pr->d;
+  if (clus < 0 || clus >= d.M || sign == 0) return -1;
+  db_lm_init(pr);
+  LMWork &w = pr->lm;
+  double2 *vr = dalloc<double2>((size_t)4 * d.R);
+  DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * d.npar, cudaMemcpyHostToDevice, d.stream));
+  db_upload_vis(pr, r, vr);
+  db_upload_vis(pr, dh, w.dbuf);
+  db_cluster_hidden(pr, clus, vr, sign, beta);
+  db_download_vis(pr, sign > 0 ? w.dbuf : vr, out);
+  db_free(vr);
+  DB_CHECK(cudaGetLastError());
+  return 0;
 }
 
 // micro-benchmark of the all-cluster predict (cost_mode 1, no output): average device time in us

@@ -18,10 +18,10 @@
 #include "rtr.h"
 #include "rtr_algo.h"
 
-void db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
-                     double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
-                     int t1, const double2 *wt, double beta, const double2 *in2, bool jte_zeroed,
-                     const double *pblk_old, bool form_hidden = false);
+int db_cluster_pass(dirac_b200_problem *pr, int k, const double *pblk_dev, const double2 *in,
+                    double2 *out, int mode, int write_out, double *jte_dev, int cost_slot, int t0,
+                    int t1, const double2 *wt, double beta, bool jte_zeroed,
+                    const double *pblk_old, bool form_hidden = false);
 void db_chunk_range(const DevProblem &d, int k, int ck, int *t0, int *t1);
 
 struct RtrWork {
@@ -244,7 +244,7 @@ void db_rtr_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
       DB_CHECK(cudaMemcpyAsync(lw.pold, pblk_dev, sizeof(double) * n8, cudaMemcpyDeviceToDevice,
                                d.stream));
     // hidden data d = beta r + f(p_old)   (lmfit.c:890-891)
-    db_cluster_pass(pr, k, pblk_dev, r, lw.dbuf, 2, 1, nullptr, 1, t0, t1, nullptr, beta, nullptr,
+    db_cluster_pass(pr, k, pblk_dev, r, lw.dbuf, 2, 1, nullptr, 1, t0, t1, nullptr, beta,
                     false, nullptr);
   }
   RtrDevEval E;
@@ -261,7 +261,7 @@ void db_rtr_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
   DB_CHECK(cudaMemcpyAsync(pblk_dev, w->h, sizeof(double) * n8, cudaMemcpyHostToDevice, d.stream));
   // residual of the chunk with the final Jones: r = d - f(p)  (lmfit.c:980-981)
   if (!hidden_ready)
-    db_cluster_pass(pr, k, pblk_dev, lw.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta, nullptr,
+    db_cluster_pass(pr, k, pblk_dev, lw.dbuf, r, 3, 1, nullptr, 1, t0, t1, nullptr, beta,
                     false, beta != 1.0 ? lw.pold : nullptr);
   db_stream_sync(d.stream);  // w->h is reused by the next visit
 }

@@ -19,7 +19,7 @@ void db_rlm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
                   int linsolv, int os, int randomize, double nulow, double nuhigh,
                   double *robust_nu, double *info, bool hidden_ready);
 bool db_cluster_needs_rowmap(const dirac_b200_problem *pr, int k);
-void db_cluster_hidden(dirac_b200_problem *pr, int k, double2 *r, int sign);
+void db_cluster_hidden(dirac_b200_problem *pr, int k, double2 *r, int sign, double beta);
 void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
                   double nu);
 void db_lbfgs_fit_minibatch(dirac_b200_problem *pr, double *p, int m, int itmax, int M, double nu);
@@ -126,7 +126,7 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
         // hybrid chunks that do not tile the interval evenly: hidden data and residual of the whole
         // cluster with the reference's row-based chunk map, the LM fits in between
         const bool hr = db_cluster_needs_rowmap(pr, cj);
-        if (hr) db_cluster_hidden(pr, cj, pr->res, +1);
+        if (hr) db_cluster_hidden(pr, cj, pr->res, +1, pr->world > 1 ? pr->beta : 1.0);
         for (int ck = 0; ck < hc[cj].nchunk; ck++) {
           const int poff = d.h_chunk_poff[hc[cj].chunk0 + ck];
           double *pblk = d.pp + poff;
@@ -193,7 +193,7 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
           final_res += info[1];
           if (pr->aug_rho) db_lm_set_aug(nullptr, nullptr, nullptr, nullptr, 0.0);
         }
-        if (hr) db_cluster_hidden(pr, cj, pr->res, -1);
+        if (hr) db_cluster_hidden(pr, cj, pr->res, -1, pr->world > 1 ? pr->beta : 1.0);
         if (init_res > 0.0) {
           nerr[cg] = (init_res - final_res) / init_res;
           if (nerr[cg] < 0.0) nerr[cg] = 0.0;

@@ -459,6 +459,50 @@ class DeviceProblem:
                               nulow, nuhigh, C.byref(nu), dptr(info))
         return p, info, nu.value
 
+    #: kernel a cluster pass ran (internal.cuh: DB_CP_*); "none": the chunk has no timeslot
+    CLUSTER_PASS_KERNELS = ("lin", "lin_grad", "split", "tile", "none")
+
+    def cluster_pass(self, clus, chunk, mode, pblk, x, write_out=True, with_jte=False,
+                     form_hidden=False, beta=1.0, pblk_old=None, wt=None, out_init=None,
+                     inplace=False):
+        """one streaming pass of chunk `chunk` of cluster clus through the LM visits' dispatch
+        (dirac_b200_cluster_pass_eval): mode 0 INIT, 1 TRIAL, 2 ADD, 3 SUB, 4 GIVEN; input x, weights
+        wt and the output vector's initial content out_init (default 0) in API layout, full interval;
+        inplace: the output vector is the input vector.
+        returns dict(kernel, out [all rows], jte [8N], cost); kernel None (out, jte, cost NaN, as the
+        hook leaves them) where the hook refuses the arguments"""
+        L = self.api.lib
+        L.dirac_b200_cluster_pass_eval.restype = C.c_int
+        L.dirac_b200_cluster_pass_eval.argtypes = ([C.c_void_p] + [C.c_int] * 6 + [C.c_double]
+                                                   + [c_double_p] * 5 + [C.c_int] + [c_double_p] * 3)
+        f64 = lambda v: None if v is None else np.ascontiguousarray(v, dtype=np.float64)
+        pblk, pblk_old, x, wt = f64(pblk), f64(pblk_old), f64(x), f64(wt)
+        out_init = np.zeros(self.n) if out_init is None else f64(out_init)
+        out = np.full(self.n, np.nan)
+        jte = np.full(8 * self.N, np.nan)
+        cost = np.full(1, np.nan)
+        opt = lambda v: dptr(v) if v is not None else None
+        k = L.dirac_b200_cluster_pass_eval(self.h, clus, chunk, mode, int(write_out), int(with_jte),
+                                           int(form_hidden), beta, dptr(pblk), opt(pblk_old),
+                                           dptr(x), opt(wt), dptr(out_init), int(inplace),
+                                           dptr(out), dptr(jte), dptr(cost))
+        return dict(kernel=None if k < 0 else self.CLUSTER_PASS_KERNELS[k], out=out, jte=jte,
+                    cost=float(cost[0]))
+
+    def cluster_hidden(self, clus, sign, beta, pp, r, dh):
+        """the row-mapped add (sign > 0) or subtract (sign < 0) of cluster clus's model at the Jones
+        pp [8 N Mt] (dirac_b200_cluster_hidden_eval) on the residual r and the hidden data dh (API
+        layout).  returns the vector it writes (hidden data, or residual), or None where refused"""
+        L = self.api.lib
+        L.dirac_b200_cluster_hidden_eval.restype = C.c_int
+        L.dirac_b200_cluster_hidden_eval.argtypes = ([C.c_void_p, C.c_int, C.c_int, C.c_double]
+                                                     + [c_double_p] * 4)
+        f64 = lambda v: np.ascontiguousarray(v, dtype=np.float64)
+        out = np.full(self.n, np.nan)
+        rv = L.dirac_b200_cluster_hidden_eval(self.h, clus, sign, beta, dptr(f64(pp)), dptr(f64(r)),
+                                              dptr(f64(dh)), dptr(out))
+        return None if rv != 0 else out
+
     def normal_eq(self, clus, chunk, pblk, xd):
         n8 = 8 * self.N
         JTJ = np.zeros((n8, n8))

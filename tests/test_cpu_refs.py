@@ -1,13 +1,16 @@
 """CPU: the plain references the GPU tests of the line model, the RTR evaluator, the IRLS update, the
-LBFGS two-loop recursion, the segmented sky staging and the minibatch band passes lean on, pinned
+LBFGS two-loop recursion, the segmented sky staging, the minibatch band passes and the LM cluster
+passes lean on, pinned
 against the restatement (oracle/liboracle.so) or the compiled reference's recorded answers before a GPU
 is involved."""
 import numpy as np
 import pytest
 
 import orcdirac
-from util import (BAND_CASES, BAND_FAULTS, U64, band_case, band_consensus, band_ref,
-                  big_cluster_sky, irls_ref, lbfgs_pairs, line_model_ref, maps_agree,
+from util import (BAND_CASES, BAND_FAULTS, CP_FAULTS, CP_RUNS, U64, band_case, band_consensus, band_ref,
+                  big_cluster_sky, chunk_offset, chunk_tiles, cluster_case, cluster_pass_ref, cp_ref_args,
+                  cp_run_applies,
+                  cluster_rowmap_ref, irls_ref, lbfgs_pairs, line_model_ref, maps_agree,
                   mult_hessian_ref, relerr, rtr_eval_ref, rtr_weights_ref, small_problem,
                   split_cluster)
 
@@ -289,5 +292,132 @@ def test_band_cases_discriminate():
                                 (np.abs(bad["res"] - good["res"]) / good["res_bound"]).max(),
                                 (np.abs(bad["grad"] - good["grad"])
                                  / np.maximum(good["grad_bound"], 1e-300)).max())
+        print("fault %s: largest error / bound %.3g" % (fault, worst))
+        assert worst > 1e3, (fault, worst)
+
+
+# ---- the LM cluster passes: util.cluster_pass_ref / cluster_rowmap_ref ----------------------------------
+def _worst(err, bound):
+    """largest err / bound (0 where both are 0)"""
+    err = np.asarray(err, dtype=np.float64)
+    return float(np.max(np.where(err == 0, 0.0, err / np.maximum(bound, 1e-300)), initial=0.0))
+
+
+def test_cluster_pass_reference_matches_compiled_reference(ref):
+    """on every (cluster, chunk) of a hybrid case whose chunks do not tile the interval evenly
+    (n7h: nchunk [1, 2, 3] over 5 timeslots), with non-zero data on flag-1 and uv-cut rows, the
+    restatement's model (x - the TRIAL output) is the reference's lm_func and its J^T e is lm_jac^T e
+    with e = x - lm_func, within the stated bounds; its row-mapped add and subtract (sign +1 / -1,
+    beta 1, r = dh = 0) are +- predict_cluster, the reference's row-mapped model of one cluster"""
+    from sagecal_b200.dirac_api import SkyModel, make_barr
+    case = cluster_case("n7h")
+    pr = case["pr"]
+    N, Nb = pr.N, pr.Nbase
+    barr, sky = make_barr(pr.sta1, pr.sta2, pr.flag), SkyModel(pr.clusters, N)
+    worst = dict(model=0.0, jte=0.0, rowmap=0.0)
+    for k in range(case["M"]):
+        for ck in range(case["nchunk"][k]):
+            t0, t1 = chunk_tiles(case, k, ck)
+            if t1 <= t0:
+                continue
+            off = chunk_offset(case, k, ck)
+            pblk = case["P_old"][off:off + 8 * N].copy()
+            r = cluster_pass_ref(case, k, ck, 1, case["x"], pblk, with_jte=True)
+            md = ref.me_data(N, Nb, t1 - t0, barr, sky, pr.coh, clus=k, tileoff=t0)
+            nn = 8 * (t1 - t0) * Nb
+            sl = slice(8 * t0 * Nb, 8 * t1 * Nb)
+            f = ref.lm_func(pblk, md, nn)
+            J = ref.lm_jac(pblk, md, nn)
+            assert not np.isnan(J).any()   # small enough to be recorded whole
+            err = np.abs((case["x"][sl] - r["out"][sl]) - f)
+            assert (err <= r["out_bound"][sl]).all(), (k, ck)
+            worst["model"] = max(worst["model"], _worst(err, r["out_bound"][sl]))
+            jte = J.T @ (case["x"][sl] - f)
+            err = np.abs(jte - r["jte"])
+            assert (err <= r["jte_bound"]).all(), (k, ck, _worst(err, r["jte_bound"]))
+            worst["jte"] = max(worst["jte"], _worst(err, r["jte_bound"]))
+            assert np.abs(r["jte"]).max() > 1e6 * r["jte_bound"].max()
+    n = 8 * pr.Nbase1
+    z = np.zeros(n)
+    for k in range(case["M"]):
+        md = ref.me_data(N, Nb, pr.tilesz, barr, sky, pr.coh, clus=k)
+        f = ref.predict_cluster(case["P_old"].copy(), md, n)
+        for sign in (1, -1):
+            o, b = cluster_rowmap_ref(case, k, sign, 1.0, case["P_old"], z, z)
+            err = np.abs(o - sign * f)
+            assert (err <= b).all(), (k, sign)
+            worst["rowmap"] = max(worst["rowmap"], _worst(err, b))
+    print("cluster_pass_ref vs compiled reference: largest error / bound: model %.3g, J^T e %.3g, "
+          "row map %.3g" % (worst["model"], worst["jte"], worst["rowmap"]))
+
+
+@pytest.mark.parametrize("beta", [0.5, 0.125, 1.0 / 64])
+def test_cluster_pass_reference_beta_identities(beta):
+    """the sharded hidden-data weight has no counterpart in the reference: pinned by identity on the
+    restatement itself.  d = INIT(beta, r, p_old) is beta r + f(p_old); the closing pass SUB(d, p,
+    recover from p_old) is d - f(p) + (1-beta) r; the row-mapped add and subtract satisfy the same
+    identities; with form_hidden, TRIAL and SUB on r equal TRIAL and SUB on the stored d"""
+    case = cluster_case("n7h")
+    N = case["N"]
+    r = case["y"]
+    worst = 0.0
+    for k, ck in ((0, 0), (1, 1), (2, 1)):
+        off = chunk_offset(case, k, ck)
+        p, po = case["P"][off:off + 8 * N], case["P_old"][off:off + 8 * N]
+        t0, t1 = chunk_tiles(case, k, ck)
+        sl = slice(8 * t0 * case["Nbase"], 8 * t1 * case["Nbase"])
+        d = cluster_pass_ref(case, k, ck, 0, r, po, beta=beta)
+        f_old = r - cluster_pass_ref(case, k, ck, 1, r, po)["out"]      # f(p_old) on the chunk
+        f_new = r - cluster_pass_ref(case, k, ck, 1, r, p)["out"]
+        err = np.abs(d["out"][sl] - (beta * r + f_old)[sl])
+        assert (err <= 2 * d["out_bound"][sl]).all()
+        worst = max(worst, _worst(err, 2 * d["out_bound"][sl]))
+        rec = cluster_pass_ref(case, k, ck, 3, d["out"], p, beta=beta, pblk_old=po)
+        want = d["out"] - f_new + (1.0 - beta) * r
+        bound = rec["out_bound"] + d["out_bound"] / beta
+        err = np.abs(rec["out"][sl] - want[sl])
+        assert (err <= bound[sl]).all(), _worst(err, bound[sl])
+        worst = max(worst, _worst(err, bound[sl]))
+        # the recovered residual is not the plain d - f(p): the (1-beta) r term is far above the bound
+        assert np.abs(rec["out"][sl] - (d["out"] - f_new)[sl]).max() > 1e6 * bound[sl].max()
+        # form_hidden on r is the pass on the stored hidden data (beta 1, as the visits use it)
+        d1 = cluster_pass_ref(case, k, ck, 0, r, po)["out"]
+        for mode in (1, 3):
+            a = cluster_pass_ref(case, k, ck, mode, r, p, form_hidden=True, pblk_old=po)
+            b = cluster_pass_ref(case, k, ck, mode, d1, p)
+            err = np.abs(a["out"][sl] - b["out"][sl])
+            assert (err <= a["out_bound"][sl] + b["out_bound"][sl]).all()
+    pp = case["P"]
+    for k in range(case["M"]):
+        dh, bd = cluster_rowmap_ref(case, k, 1, beta, case["P_old"], r, np.zeros_like(r))
+        m_old = cluster_rowmap_ref(case, k, 1, 1.0, case["P_old"], np.zeros_like(r), r)[0]
+        assert (np.abs(dh - (beta * r + m_old)) <= bd).all()
+        o, bo = cluster_rowmap_ref(case, k, -1, beta, pp, r, dh)
+        m_new = cluster_rowmap_ref(case, k, 1, 1.0, pp, np.zeros_like(r), r)[0]
+        err = np.abs(o - (dh - m_new + (1.0 - beta) * r))
+        assert (err <= bo).all()
+    print("beta %g: largest error / bound %.3g" % (beta, worst))
+
+
+def _cp_runs(case):
+    """(k, ck, name, run) of the cluster-pass checks of tests/test_gpu_cluster_pass.py on a case"""
+    return [(k, ck, name, kw) for k in range(case["M"]) for ck in range(case["nchunk"][k])
+            for name, kw in CP_RUNS if cp_run_applies(case, name, kw)]
+
+
+def test_cluster_pass_cases_discriminate():
+    """every deliberate fault of CP_FAULTS, applied to cluster_pass_ref, moves some quantity of some GPU
+    case (test_gpu_cluster_pass.py) past its bound by more than 10^3: the cases can see it"""
+    cases = [cluster_case(n) for n in ("n2", "n24", "n9e", "n9r")]
+    for fault in CP_FAULTS:
+        worst = 0.0
+        for case in cases:
+            for k, ck, name, kw in _cp_runs(case):
+                a = cp_ref_args(case, k, ck, kw)
+                good = cluster_pass_ref(case, k, ck, **a)
+                bad = cluster_pass_ref(case, k, ck, fault=fault, **a)
+                worst = max(worst, _worst(np.abs(bad["out"] - good["out"]), good["out_bound"]),
+                            _worst(abs(bad["cost"] - good["cost"]), good["cost_bound"]),
+                            _worst(np.abs(bad["jte"] - good["jte"]), good["jte_bound"]))
         print("fault %s: largest error / bound %.3g" % (fault, worst))
         assert worst > 1e3, (fault, worst)

@@ -788,3 +788,319 @@ def band_ref(case, p, nu, y=None, z=None, rho=None, fault=None):
         grad = grad + gc
     return dict(cost=cost, res=res, grad=grad, res_bound=res_bound, cost_bound=cost_bound,
                 grad_bound=grad_bound)
+
+
+# ---- the LM cluster passes (k_cluster_pass_lin, k_cluster_pass_split, k_cluster_pass, k_cluster_rowmap)
+#: c of the element-wise bound c u (|beta v| + |Jp||C||Jq|^T) of one model added to or subtracted from
+#: a vector: two 2x2 complex products and the add, a few roundings each
+CP_C = 10.0
+
+#: (N, timeslots, nchunk of the clusters) of the cluster-pass cases (tests/test_gpu_cluster_pass.py)
+CP_CASES = {
+    "n7h": (7, 5, [1, 2, 3]),
+    "n2": (2, 3, [1, 2]),
+    "n23": (23, 5, [1, 2, 3]),
+    "n24": (24, 5, [1, 2, 3]),
+    "n9e": (9, 3, [1, 4]),
+    "n9r": (9, 64, [1, 2]),
+    "n62": (62, 120, [1]),
+    "n512": (512, 2, [1]),
+    "n639": (639, 2, [1]),
+    "n640": (640, 2, [1]),
+}
+
+#: deliberate faults cluster_pass_ref can apply to itself (tests/test_cpu_refs.py)
+CP_FAULTS = ("model_on_flagged", "beta_on_model", "gamma_one_minus_beta", "chunk_shift",
+             "jq_not_hermitian", "jte_without_q", "drop_last_group", "drop_last_slice",
+             "weights_once")
+
+
+def cluster_case(name, seed=61):
+    """one resident problem of CP_CASES[name]: random-phase coherencies, data = model at the true
+    Jones plus noise, NON-ZERO on flagged rows; random flag-1 and uv-cut (flag 2) rows, one station
+    (N > 2) and one timeslot (T > 1) fully flagged.  Jones: P near the truth, P_old farther from it;
+    wt positive sqrt-weights, y a second input vector, out_init a non-zero vector (API layout)."""
+    N, T, nchunk = CP_CASES[name]
+    rng = np.random.default_rng(seed + 3 * N + T)
+    M = len(nchunk)
+    pr = synth.make_problem(N=N, M=M, tilesz=T, seed=seed + N, nchunk=nchunk, flag_frac=0.0,
+                            uvcut_frac=0.0, with_data=False)
+    R, Nb = pr.Nbase1, pr.Nbase
+    fl = np.zeros(R, dtype=np.uint8)
+    uu = rng.uniform(0, 1, R)
+    fl[uu < 0.06] = 1
+    fl[(uu >= 0.06) & (uu < 0.1)] = 2
+    if N > 2:
+        s = N // 2
+        fl[(pr.sta1 == s) | (pr.sta2 == s)] = 1
+    if T > 1:
+        t = T // 2
+        fl[t * Nb:(t + 1) * Nb] = 2
+    pr.flag = fl
+    amp = rng.lognormal(0.0, 0.5, (R, M, 4))
+    coh = amp * np.exp(2j * np.pi * rng.uniform(0, 1, (R, M, 4)))
+    pr.coh = coh.reshape(-1)
+    x = synth.apply_jones(pr.coh, pr.jones_true, pr.sta1, pr.sta2, N, pr.nchunk)
+    x = x + 0.01 * np.median(np.abs(x)) * rng.normal(0, 1, x.shape)
+    pr.x = x
+    m = 8 * N * pr.Mt
+    return dict(pr=pr, name=name, N=N, Nbase=Nb, tilesz=T, M=M, nchunk=list(pr.nchunk),
+                sta1=pr.sta1, sta2=pr.sta2, flag=fl, coh=coh, x=x,
+                y=rng.normal(0, 1, x.shape) * np.median(np.abs(x)),
+                wt=rng.uniform(0.2, 1.3, x.shape), out_init=rng.normal(0, 1, x.shape),
+                P=pr.jones_true + 1e-3 * rng.normal(0, 1, m),
+                P_old=pr.jones_true + 0.1 * rng.normal(0, 1, m))
+
+
+def chunk_offset(case, k, ck):
+    """offset of the Jones block of (cluster k, chunk ck) in the parameter vector"""
+    return 8 * case["N"] * (int(sum(case["nchunk"][:k])) + ck)
+
+
+def chunk_tiles(case, k, ck):
+    """timeslots [t0, t1) of chunk ck of cluster k (the LM fits' ranges, lmfit.c:893-905)"""
+    T = case["tilesz"]
+    tc = -(-T // case["nchunk"][k])
+    t0 = min(ck * tc, T)
+    return t0, min(t0 + tc, T)
+
+
+def _cplx(v):
+    """API layout [8 R] -> [R, 2, 2] complex"""
+    a = np.asarray(v, dtype=np.float64).reshape(-1, 4, 2)
+    return (a[..., 0] + 1j * a[..., 1]).reshape(-1, 2, 2)
+
+
+def _split(z):
+    """[R, 2, 2] complex -> [R, 8] real (re, im per component)"""
+    return _api_layout(z).reshape(-1, 8)
+
+
+def _model(J, C, p, q, fault=None):
+    """Jp C Jq^H and its magnitude companion |Jp||C||Jq|^T, per row"""
+    Jp, Jq = J[p], J[q]
+    Jh = Jq if fault == "jq_not_hermitian" else np.conj(np.swapaxes(Jq, -1, -2))
+    m = _mm2(_mm2(Jp, C), Jh)
+    A = _mm2(_mm2(np.abs(Jp), np.abs(C)), np.swapaxes(np.abs(Jq), -1, -2))
+    return m, A
+
+
+def cluster_pass_ref(case, k, ck, mode, x, pblk, write_out=True, with_jte=False, form_hidden=False,
+                     beta=1.0, pblk_old=None, wt=None, out_init=None, inplace=False, fault=None):
+    """plain per-row float64 restatement of one LM cluster pass (ClusterPassArgs, kernels_stream.cu)
+    of cluster k, chunk ck over its timeslots [t0, t1), input vector x (API layout, full interval):
+      model  m = Jp C Jq^H at pblk, zero on flag-1 and uv-cut rows; m_old the same at pblk_old
+      v      x, or with form_hidden the hidden data beta x + m_old formed per row
+      mode 0 INIT   d = beta v + m -> out, e = d - m
+           1 TRIAL  e = v - m -> out
+           2 ADD    out = beta v + m
+           3 SUB    out = v - m, with pblk_old (not form_hidden) the recovered old residual added:
+                    + (1-beta)/beta (v - m_old)
+           4 GIVEN  e = v -> out
+      cost   ||e||^2, or ||wt.e||^2 (modes 0, 1, 4), over every row of the chunk
+      J^T e  station sums over the chunk's unflagged rows of E Jq C^H (station p) and E^H Jp C
+             (station q), E = e or wt^2.e, in the parameter layout
+    Rows outside the chunk, and every row without write_out, keep the output vector's content (x
+    itself when inplace).  The a-priori bounds of any float64 evaluation:
+      out_bound   CP_C u (|beta v| + |Jp||C||Jq|^T), plus CP_C u (|beta x| + |m_old|-companion) where
+                  the second model forms v, plus (1-beta)/beta CP_C u (|v| + companion) to recover
+      cost_bound  per-term rounding, the residual error through 2|e|, the summation
+      jte_bound   n u sum |E||J||C| plus the residual error through |J||C|, per component
+    Sums in long double.  `fault` (one of CP_FAULTS) makes the restatement deliberately wrong.
+    returns dict(out, out_bound, cost, cost_bound, jte, jte_bound, rows=(r0, r1))"""
+    N, Nb, T = case["N"], case["Nbase"], case["tilesz"]
+    R = Nb * T
+    u = U64
+    t0, t1 = chunk_tiles(case, k, ck)
+    if fault == "chunk_shift":
+        t0, t1 = min(t0 + 1, T), min(t1 + 1, T)
+    r0, r1 = t0 * Nb, t1 * Nb
+    rows = np.arange(r0, r1)
+    keep = np.ones(r1 - r0, dtype=bool)   # rows a faulty kernel would still visit
+    if fault == "drop_last_group":
+        keep &= (rows % Nb) < ((Nb - 1) // 256) * 256
+    elif fault == "drop_last_slice":
+        keep &= rows < max(r0, r1 - Nb)
+    p, q = case["sta1"][r0:r1], case["sta2"][r0:r1]
+    fl = case["flag"][r0:r1] != 0
+    C = case["coh"].reshape(R, case["M"], 2, 2)[r0:r1, k]
+    v = _cplx(x)[r0:r1]
+    vw = np.abs(v)
+    m, A = _model(_jones(pblk, N), C, p, q, fault)
+    old = pblk_old is not None and (form_hidden or mode == 3)
+    if old:
+        mo, Ao = _model(_jones(pblk_old, N), C, p, q, fault)
+    if fault != "model_on_flagged":
+        m[fl] = 0.0
+        A[fl] = 0.0
+        if old:
+            mo[fl] = 0.0
+            Ao[fl] = 0.0
+    cu = CP_C * u
+    dv = np.zeros(v.shape)
+    if form_hidden:
+        v = (v + beta * mo) if fault == "beta_on_model" else (beta * v + mo)
+        dv = cu * (np.abs(beta) * vw + Ao)
+    add = lambda a, b: (a + beta * b) if fault == "beta_on_model" else (beta * a + b)
+    e = None
+    if mode in (0, 2):
+        o = add(v, m)
+        do = cu * (np.abs(beta) * np.abs(v) + A) + np.abs(beta) * dv
+        if mode == 0:
+            e = o - m
+    elif mode == 4:
+        e = o = v
+        do = dv
+    else:
+        e = v - m
+        o = e
+        do = cu * (np.abs(v) + A) + dv
+        if mode == 3 and pblk_old is not None and not form_hidden:
+            g = (1.0 - beta) if fault == "gamma_one_minus_beta" else (1.0 - beta) / beta
+            o = e + g * (v - mo)
+            do = do + abs((1.0 - beta) / beta) * cu * (np.abs(v) + Ao)
+    de = do if e is not None else None
+    base = np.array(x if inplace else (np.zeros(8 * R) if out_init is None else out_init),
+                    dtype=np.float64)
+    out = base.copy().reshape(R, 8)
+    out_bound = np.zeros((R, 8))
+    if write_out:
+        sel = rows[keep]
+        out[sel] = _split(o)[keep]
+        out_bound[sel] = np.repeat(do.reshape(-1, 4)[keep], 2, axis=1)
+    res = dict(out=out.reshape(-1), out_bound=out_bound.reshape(-1), cost=0.0, cost_bound=0.0,
+               jte=np.zeros(8 * N), jte_bound=np.zeros(8 * N), rows=(r0, r1))
+    if mode not in (0, 1, 4):
+        return res
+    w = np.ones((r1 - r0, 8)) if wt is None else np.asarray(wt, dtype=np.float64).reshape(R, 8)[r0:r1]
+    e8 = _split(e)
+    de8 = np.repeat(de.reshape(-1, 4), 2, axis=1)
+    terms = ((w * e8) ** 2)[keep]
+    res["cost"] = lsum(terms)
+    res["cost_bound"] = (lsum(3 * u * terms) + lsum((2 * w * w * np.abs(e8) * de8 + (w * de8) ** 2)[keep])
+                         + terms.size * u * lsum(terms))
+    if with_jte:
+        use = keep & ~fl
+        w2 = w if fault == "weights_once" else w * w
+        E8 = np.where(use[:, None], w2 * e8, 0.0)
+        Ea8 = np.abs(E8)
+        Ed8 = np.where(use[:, None], w * w * de8, 0.0)
+        to2 = lambda a: (a[:, 0::2] + 1j * a[:, 1::2]).reshape(-1, 2, 2)
+        E = to2(E8)
+        Ea = (Ea8[:, 0::2] + Ea8[:, 1::2]).reshape(-1, 2, 2)
+        Ed = (Ed8[:, 0::2] + Ed8[:, 1::2]).reshape(-1, 2, 2)
+        J = _jones(pblk, N)
+        aJ = np.abs(J)
+        H = lambda X: np.conj(np.swapaxes(X, -1, -2))
+        Tt = lambda X: np.swapaxes(X, -1, -2)
+        Ca = np.abs(C)
+        nt = t1 - t0
+        G = _scatter2(p, _mm2(_mm2(E, J[q]), H(C)), N)
+        Ga = _scatter2(p, _mm2(_mm2(Ea, aJ[q]), Tt(Ca)), N)
+        Gd = _scatter2(p, _mm2(_mm2(Ed, aJ[q]), Tt(Ca)), N)
+        if fault != "jte_without_q":
+            G += _scatter2(q, _mm2(_mm2(H(E), J[p]), C), N)
+        Ga += _scatter2(q, _mm2(_mm2(Tt(Ea), aJ[p]), Ca), N)
+        Gd += _scatter2(q, _mm2(_mm2(Tt(Ed), aJ[p]), Ca), N)
+        nsum = 8 * max(N - 1, 1) * max(nt, 1) + 16
+        res["jte"] = _api_layout(G)
+        res["jte_bound"] = np.repeat((nsum * u * Ga + Gd).reshape(-1), 2)
+    return res
+
+
+def cluster_rowmap_ref(case, k, sign, beta, pp, r, dh, fault=None):
+    """plain per-row float64 restatement of db_cluster_hidden (k_cluster_rowmap) for cluster k at the
+    full Jones vector pp, the chunk of a row by the row map (synth.chunk_index, as line_model_ref):
+      sign > 0  hidden data  beta r + m
+      sign < 0  residual     dh - m (+ (1-beta) r when beta != 1)
+    m zero on flag-1 and uv-cut rows.  returns (out, bound) over every row, bound
+    CP_C u (|beta r| + |dh| + |(1-beta) r| + |Jp||C||Jq|^T) of the terms that enter"""
+    N, R = case["N"], case["Nbase"] * case["tilesz"]
+    rows = np.arange(R)
+    nch = case["nchunk"][k]
+    px = synth.chunk_index(rows, R, nch)
+    J = _jones(np.asarray(pp)[chunk_offset(case, k, 0):chunk_offset(case, k, nch)], N * nch)
+    idx = px * N
+    C = case["coh"].reshape(R, case["M"], 2, 2)[:, k]
+    m, A = _model(J, C, idx + case["sta1"], idx + case["sta2"], fault)
+    if fault != "model_on_flagged":
+        fl = case["flag"] != 0
+        m[fl] = 0.0
+        A[fl] = 0.0
+    rv, dv = _cplx(r), _cplx(dh)
+    if sign > 0:
+        o = (rv + beta * m) if fault == "beta_on_model" else (beta * rv + m)
+        b = CP_C * U64 * (abs(beta) * np.abs(rv) + A)
+    else:
+        o = dv - m
+        b = CP_C * U64 * (np.abs(dv) + A)
+        if beta != 1.0:
+            o = o + (1.0 - beta) * rv
+            b = b + CP_C * U64 * abs(1.0 - beta) * np.abs(rv)
+    return _api_layout(o), np.repeat(b.reshape(-1), 2)
+
+
+#: the passes each cluster-pass case runs: (name, arguments); old: the visit's entry Jones P_old as
+#: pblk_old, wt: the case's weights.  init/trial with and without output, J^T e and weights; the trial
+#: that forms the hidden data with J^T e (k_cluster_pass_lin<true> reloads the old Jones per row) and
+#: without it (the last trial, which writes the residual); ADD with beta; SUB plain, recovering at beta
+#: 1/2, 1/8, 1/64 and forming the hidden data in place; the given-residual pass of the OS-LM
+CP_RUNS = [
+    ("init", dict(mode=0, write_out=True, with_jte=True)),
+    ("init_beta", dict(mode=0, write_out=True, with_jte=True, beta=0.125)),
+    ("init_quiet", dict(mode=0, write_out=False)),
+    ("init_beta_out", dict(mode=0, write_out=True, beta=0.125)),
+    ("trial", dict(mode=1, write_out=True, with_jte=True)),
+    ("trial_quiet", dict(mode=1, write_out=False)),
+    ("trial_wt", dict(mode=1, write_out=True, with_jte=True, wt=True)),
+    ("trial_wt_cost", dict(mode=1, write_out=False, wt=True)),
+    ("trial_form", dict(mode=1, write_out=False, with_jte=True, form_hidden=True, old=True)),
+    ("trial_form_last", dict(mode=1, write_out=True, form_hidden=True, old=True)),
+    ("add", dict(mode=2, write_out=True, beta=0.125)),
+    ("add_quiet", dict(mode=2, write_out=False)),
+    ("sub", dict(mode=3, write_out=True)),
+    ("sub_rec2", dict(mode=3, write_out=True, beta=0.5, old=True)),
+    ("sub_rec8", dict(mode=3, write_out=True, beta=0.125, old=True)),
+    ("sub_rec64", dict(mode=3, write_out=True, beta=1.0 / 64, old=True)),
+    ("sub_form_inplace", dict(mode=3, write_out=True, form_hidden=True, old=True, inplace=True)),
+    ("given", dict(mode=4, write_out=True, with_jte=True, wt=True)),
+]
+
+
+def cp_lin_fits(N, Nbase):
+    """whether the linear-mapped pass takes the array (kernels_stream.cu: cluster_pass_lin_fits): 8N
+    station sums next to a 5-stage ring in 200 KB of shared memory, at most 1024 baseline groups"""
+    return 5 * 8 * 256 * 16 + 8 * ((8 * N + 1) & ~1) + 40 <= 200 * 1024 and (Nbase + 255) // 256 <= 1024
+
+
+def cp_run_applies(case, name, kw):
+    """form_hidden runs only where the linear-mapped kernel takes the array; the given-residual pass
+    at n24 and n640"""
+    if kw.get("form_hidden") and not cp_lin_fits(case["N"], case["Nbase"]):
+        return False
+    return kw["mode"] != 4 or case["name"] in ("n24", "n640")
+
+
+def cp_ref_args(case, k, ck, kw):
+    """the arguments of cluster_pass_ref (and of DeviceProblem.cluster_pass) for run kw on (k, ck)"""
+    N = case["N"]
+    off = chunk_offset(case, k, ck)
+    return dict(mode=kw["mode"], x=case["x"], pblk=case["P"][off:off + 8 * N],
+                write_out=kw.get("write_out", True), with_jte=kw.get("with_jte", False),
+                form_hidden=kw.get("form_hidden", False), beta=kw.get("beta", 1.0),
+                pblk_old=case["P_old"][off:off + 8 * N] if kw.get("old") else None,
+                wt=case["wt"] if kw.get("wt") else None, out_init=case["out_init"],
+                inplace=kw.get("inplace", False))
+
+
+def cp_expected_kernel(case, k, ck, kw):
+    """the kernel db_launch_cluster_pass picks for run kw (kernels_stream.cu)"""
+    t0, t1 = chunk_tiles(case, k, ck)
+    if t1 <= t0:
+        return "none"
+    fits = cp_lin_fits(case["N"], case["Nbase"])
+    if not kw.get("with_jte") or kw["mode"] in (2, 3):
+        return "lin" if (fits and not kw.get("wt")) else "tile"
+    if kw["mode"] == 4 or kw.get("wt") or not fits:
+        return "split"
+    return "lin_grad"
