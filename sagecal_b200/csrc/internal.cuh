@@ -293,6 +293,8 @@ struct StreamAllArgs {
   const short2 *blpq;
   double2 *out;              // MODE 0
   double2 *E0, *E1, *E2;     // MODE 1
+  double *poly_part;         // MODE 1, partial == 0: per-CTA sums of the line quartic, [5][grid]
+                             // (null: not formed)
   double *partials, *cost;
   unsigned int *counter;
   long long R;
@@ -336,7 +338,8 @@ struct AssembleArgs {
 
 // test / tuning options (dirac_b200_set_option): 0 = default
 enum { DB_OPT_CP_ROWS = 0, DB_OPT_LINE_DIRECT = 1, DB_OPT_OS_CONSISTENT = 2,
-       DB_OPT_RTR_NU_UNJOINED = 3, DB_OPT_ADMM_LM = 4, DB_OPT_COUNT = 8 };
+       DB_OPT_RTR_NU_UNJOINED = 3, DB_OPT_ADMM_LM = 4, DB_OPT_SWEEP_RESIDUAL = 5,
+       DB_OPT_COUNT = 8 };
 int db_opt(int id);
 int db_sm_count();  // SMs of the current device
 // slices of the time axis the linear-mapped gradient pass may use (sizes LMWork::jte_part)
@@ -398,7 +401,12 @@ void db_launch_cost_window_tma(const StreamAllArgs *a, cudaStream_t st);
 int db_band_nblocks(int Nbase, int tilesz, int nchan);
 void db_launch_band_tma(const StreamAllArgs *a, int nchan, cudaStream_t st);
 void db_launch_band_tma(const StreamAllArgs *a, int nchan, cudaStream_t st);
-void db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st);
+// returns the grid (the columns of a->poly_part it wrote, when set)
+unsigned db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st);
+// k_line_poly_finish: the five quartic coefficients from the [5][nparts] per-CTA sums of
+// k_stream_all<1>, into out[0..4]
+void db_launch_line_poly_finish(const double *part, unsigned nparts, double *partials, double *out,
+                                unsigned int *counter, cudaStream_t st);
 // (TB, NST, WARPS) of the last k_stream_all<1> launch since the reset (-1 each: none)
 void db_line_setup_shape_reset();
 void db_line_setup_shape(int *shape);

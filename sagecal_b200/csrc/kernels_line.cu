@@ -73,23 +73,10 @@ k_line_eval(const double2 *__restrict__ E0, const double2 *__restrict__ E1,
   grid_reduce_sum_l(s, partials, out, counter);
 }
 
-// Gaussian cost along the line is the quartic sum |E0 - a E1 - a^2 E2|^2 = c0 + c1 a + ... + c4 a^4:
-// the five coefficients in one deterministic reduction (per-CTA partials, fixed-order final sum)
-__global__ void __launch_bounds__(256)
-k_line_poly(const double2 *__restrict__ E0, const double2 *__restrict__ E1,
-            const double2 *__restrict__ E2, long long n4, double *partials, double *out,
-            unsigned int *counter) {
-  double c[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4;
-       i += (long long)gridDim.x * blockDim.x) {
-    const double2 e0 = E0[i], e1 = E1[i], e2 = E2[i];
-    c[0] = fma(e0.x, e0.x, fma(e0.y, e0.y, c[0]));
-    c[1] = fma(e0.x, e1.x, fma(e0.y, e1.y, c[1]));
-    c[2] = fma(e1.x, e1.x, fma(e1.y, e1.y, c[2]));
-    c[2] = fma(-2.0 * e0.x, e2.x, fma(-2.0 * e0.y, e2.y, c[2]));
-    c[3] = fma(e1.x, e2.x, fma(e1.y, e2.y, c[3]));
-    c[4] = fma(e2.x, e2.x, fma(e2.y, e2.y, c[4]));
-  }
+// the five sums c[] of every thread of a 256-thread grid -> out[0..4] (per-CTA partials, fixed-order
+// final sum), with c1 = -2 sum E0.E1 and c3 = 2 sum E1.E2
+__device__ __forceinline__ void poly_grid_reduce(const double *c, double *partials, double *out,
+                                                 unsigned int *counter) {
   __shared__ double ws[5][8];
   __shared__ bool is_last;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -118,6 +105,53 @@ k_line_poly(const double2 *__restrict__ E0, const double2 *__restrict__ E1,
     out[threadIdx.x] = s;
     if (threadIdx.x == 0) *counter = 0;
   }
+}
+
+// Gaussian cost along the line is the quartic sum |E0 - a E1 - a^2 E2|^2 = c0 + c1 a + ... + c4 a^4:
+// the five coefficients in one deterministic reduction.  Sharded runs form E0 only after the sum over
+// the ranks, so they take this pass; one GPU folds the sums into k_stream_all<1> (k_line_poly_finish)
+__global__ void __launch_bounds__(256)
+k_line_poly(const double2 *__restrict__ E0, const double2 *__restrict__ E1,
+            const double2 *__restrict__ E2, long long n4, double *partials, double *out,
+            unsigned int *counter) {
+  double c[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4;
+       i += (long long)gridDim.x * blockDim.x) {
+    const double2 e0 = E0[i], e1 = E1[i], e2 = E2[i];
+    c[0] = fma(e0.x, e0.x, fma(e0.y, e0.y, c[0]));
+    c[1] = fma(e0.x, e1.x, fma(e0.y, e1.y, c[1]));
+    c[2] = fma(e1.x, e1.x, fma(e1.y, e1.y, c[2]));
+    c[2] = fma(-2.0 * e0.x, e2.x, fma(-2.0 * e0.y, e2.y, c[2]));
+    c[3] = fma(e1.x, e2.x, fma(e1.y, e2.y, c[3]));
+    c[4] = fma(e2.x, e2.x, fma(e2.y, e2.y, c[4]));
+  }
+  poly_grid_reduce(c, partials, out, counter);
+}
+
+// the quartic from the per-CTA sums k_stream_all<1> left in part ([5][nparts]): 40 B per CTA of the
+// line-model pass instead of a second read of E0, E1 and E2
+__global__ void __launch_bounds__(256)
+k_line_poly_finish(const double *__restrict__ part, unsigned nparts, double *partials, double *out,
+                   unsigned int *counter) {
+  double c[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < nparts; i += gridDim.x * blockDim.x)
+#pragma unroll
+    for (int j = 0; j < 5; j++) c[j] += part[(size_t)j * nparts + i];
+  poly_grid_reduce(c, partials, out, counter);
+}
+
+// out = sum |v|^2 over n4 double2 (the cost of a residual already in HBM)
+__global__ void __launch_bounds__(256)
+k_sumsq(const double2 *__restrict__ v, long long n4, double *partials, double *out,
+        unsigned int *counter) {
+  double s = 0.0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4;
+       i += (long long)gridDim.x * blockDim.x) {
+    const double2 e = v[i];
+    s = fma(e.x, e.x, s);
+    s = fma(e.y, e.y, s);
+  }
+  grid_reduce_sum_l(s, partials, out, counter);
 }
 
 // res = E0 - alpha E1 - alpha^2 E2
@@ -238,6 +272,14 @@ void db_launch_cluster_rowmap(const double2 *coh_k, const double2 *in, const dou
 void db_launch_line_poly(const double2 *E0, const double2 *E1, const double2 *E2, long long n4,
                          double *partials, double *out, unsigned int *counter, cudaStream_t st) {
   k_line_poly<<<192, 256, 0, st>>>(E0, E1, E2, n4, partials, out, counter);
+}
+void db_launch_line_poly_finish(const double *part, unsigned nparts, double *partials, double *out,
+                                unsigned int *counter, cudaStream_t st) {
+  k_line_poly_finish<<<192, 256, 0, st>>>(part, nparts, partials, out, counter);
+}
+void db_launch_sumsq(const double2 *v, long long n4, double *partials, double *out,
+                     unsigned int *counter, cudaStream_t st) {
+  k_sumsq<<<LINE_GRID, 256, 0, st>>>(v, n4, partials, out, counter);
 }
 void db_launch_line_residual(const double2 *E0, const double2 *E1, const double2 *E2, double2 *res,
                              long long n4, double alpha, cudaStream_t st) {

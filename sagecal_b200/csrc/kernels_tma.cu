@@ -2,7 +2,8 @@
 // shared-memory stages):
 //   MODE 0  model over all clusters, residual / cost      (predict_threadfn_withgain_full,
 //           lmfit.c:611-688, plus cost_func / robust_cost_func, robust_lbfgs.c:674-726)
-//   MODE 1  line model V0,V1,V2 -> E0,E1,E2 of the LBFGS line search (kernels_line.cu)
+//   MODE 1  line model V0,V1,V2 -> E0,E1,E2 of the LBFGS line search (kernels_line.cu), and on one
+//           GPU the per-CTA sums of the Gaussian cost's quartic along the line
 //   MODE 2  MODE 0 over a row window [w_lo, w_hi) of the launched timeslots: the cost and residual
 //           of the minibatch LBFGS (robust_cost_func_batch, robust_batchmode_lbfgs.c:822-846); rows
 //           of the first and last timeslot outside the window are neither written nor summed
@@ -163,6 +164,9 @@ k_stream_all(StreamAllArgs a) {
   }
   __syncthreads();
   double cost = 0.0;
+  // MODE 1 on one GPU: the Gaussian cost along the line, sum |E0 - a E1 - a^2 E2|^2, is a quartic
+  // whose five sums (k_line_poly's) are taken here from the E0, E1, E2 this warp stores
+  double cq[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
   if (w == 0 && valid) {
     for (int ww = 1; ww < WARPS; ww++)
 #pragma unroll
@@ -202,12 +206,30 @@ k_stream_all(StreamAllArgs a) {
             }
           } else {
             const double2 xv = ld_stream(a.x + ix);
-            st_stream(a.E0 + ix, a.partial ? m : csub(xv, m));
-            st_stream(a.E1 + ix, fl ? z : V1[i][c]);
-            st_stream(a.E2 + ix, fl ? z : V2[i][c]);
+            const double2 e0 = a.partial ? m : csub(xv, m);
+            const double2 e1 = fl ? z : V1[i][c], e2 = fl ? z : V2[i][c];
+            st_stream(a.E0 + ix, e0);
+            st_stream(a.E1 + ix, e1);
+            st_stream(a.E2 + ix, e2);
+            if (a.poly_part) {
+              cq[0] = fma(e0.x, e0.x, fma(e0.y, e0.y, cq[0]));
+              cq[1] = fma(e0.x, e1.x, fma(e0.y, e1.y, cq[1]));
+              cq[2] = fma(e1.x, e1.x, fma(e1.y, e1.y, cq[2]));
+              cq[2] = fma(-2.0 * e0.x, e2.x, fma(-2.0 * e0.y, e2.y, cq[2]));
+              cq[3] = fma(e1.x, e2.x, fma(e1.y, e2.y, cq[3]));
+              cq[4] = fma(e2.x, e2.x, fma(e2.y, e2.y, cq[4]));
+            }
           }
         }
       }
+    }
+  }
+  if (MODE == 1 && a.poly_part && w == 0) {
+    // per-CTA sums in lane order; k_line_poly_finish adds the CTAs in index order (deterministic)
+#pragma unroll
+    for (int j = 0; j < 5; j++) {
+      const double v = warp_sum(cq[j]);
+      if (lane == 0) a.poly_part[(size_t)j * gridDim.x + blockIdx.x] = v;
     }
   }
   if (MODE != 1 && a.cost_mode) {
@@ -236,7 +258,7 @@ k_stream_all(StreamAllArgs a) {
 static int g_line_shape[3] = {-1, -1, -1};  // shape of the last line-model launch (tests)
 
 template <int MODE, int TB, int NST, int WARPS>
-static void launch_cfg(const StreamAllArgs *a, cudaStream_t st) {
+static unsigned launch_cfg(const StreamAllArgs *a, cudaStream_t st) {
   if (MODE == 1) {
     g_line_shape[0] = TB;
     g_line_shape[1] = NST;
@@ -255,6 +277,7 @@ static void launch_cfg(const StreamAllArgs *a, cudaStream_t st) {
     configured = true;
   }
   k_stream_all<MODE, TB, NST, WARPS><<<grid, WARPS * 32, smem, st>>>(*a);
+  return grid;
 }
 
 extern "C" {
@@ -271,14 +294,14 @@ void db_launch_predict_tma(const StreamAllArgs *a, cudaStream_t st) {
 void db_launch_cost_window_tma(const StreamAllArgs *a, cudaStream_t st) {
   launch_cfg<2, 2, 2, 3>(a, st);
 }
-void db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st) {
+unsigned db_launch_line_setup_tma(const StreamAllArgs *a, cudaStream_t st) {
   // one row per item keeps the three accumulated polynomials of the line model at 24 registers
   // pairs (222 -> ~170 registers: 7.5 % -> 12 % resident warps, ncu r02).  Splitting the clusters
   // of an item over warps only pays while the grid is short of warps (62 stations: 7200 items);
   // a large array has plenty (512 stations: 490 k items) and skips the cross-warp combine.
   const long long items = (long long)((a->Nbase + 31) / 32) * a->tilesz;
-  if (items >= 64ll * db_sm_count()) launch_cfg<1, 1, 4, 1>(a, st);
-  else launch_cfg<1, 1, 2, 3>(a, st);
+  if (items >= 64ll * db_sm_count()) return launch_cfg<1, 1, 4, 1>(a, st);
+  return launch_cfg<1, 1, 2, 3>(a, st);
 }
 void db_line_setup_shape_reset() { g_line_shape[0] = g_line_shape[1] = g_line_shape[2] = -1; }
 void db_line_setup_shape(int *shape) {

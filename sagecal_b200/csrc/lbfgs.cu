@@ -56,10 +56,13 @@ static void line_alloc(dirac_b200_problem *pr) {
   if (pr->E0) return;
   DevProblem &d = pr->d;
   const size_t n = (size_t)4 * d.R;
-  // one allocation: the three parts of the line model travel in ONE all-reduce when sharded
-  pr->E0 = (decltype(pr->E0))db_malloc(sizeof(double2) * n * 3);
+  const size_t nb = (size_t)db_stream_all_nblocks(d.Nbase, d.tilesz);
+  // one allocation: the three parts of the line model travel in ONE all-reduce when sharded; the
+  // per-CTA quartic sums of a single-GPU pass follow them
+  pr->E0 = (decltype(pr->E0))db_malloc(sizeof(double2) * n * 3 + sizeof(double) * 5 * nb);
   pr->E1 = pr->E0 + n;
   pr->E2 = pr->E1 + n;
+  pr->poly_part = reinterpret_cast<double *>(pr->E2 + n);
 }
 
 // line model along pk from xk (both device vectors)
@@ -73,6 +76,12 @@ static void line_setup(LbfgsCtx *c, const double *xk, const double *pk) {
   s.chunk_poff = d.chunk_poff; s.blpq = d.blpq; s.E0 = pr->E0; s.E1 = pr->E1; s.E2 = pr->E2;
   s.R = d.R; s.N = d.N; s.Nbase = d.Nbase; s.tilesz = d.tilesz; s.M = d.M;
   s.partial = (pr->world > 1) ? 1 : 0;  // 1: the raw sums V0,V1,V2 of the local clusters
+  // the Gaussian cost along the line is a quartic in alpha: five sums, then every cost evaluation of
+  // the line search is arithmetic on the host.  One GPU has E0 in the line-model pass and takes the
+  // sums there; sharded runs form E0 after the all-reduce and sum with k_line_poly
+  const bool want_poly = !c->robust && !db_opt(DB_OPT_LINE_DIRECT);
+  const bool fold_poly = want_poly && pr->world <= 1;
+  s.poly_part = fold_poly ? pr->poly_part : nullptr;
   if (db_overlap_available(pr) && d.tilesz >= 8) {
     // Sharded: the kernel runs in time chunks; each chunk's 12 slices (3 vectors x 4 polarisation
     // planes) are summed over the ranks on the communication stream while the next chunk is computed
@@ -116,9 +125,14 @@ static void line_setup(LbfgsCtx *c, const double *xk, const double *pk) {
     db_count_launch(1);
   } else {
     db_prof_begin(7, (double)d.R * (64.0 * d.M + 65.0 + 192.0), d.stream);
-    db_launch_line_setup_tma(&s, d.stream);
+    const unsigned nparts = db_launch_line_setup_tma(&s, d.stream);
     db_prof_end(d.stream);
     db_count_launch(1);
+    if (fold_poly) {
+      db_launch_line_poly_finish(pr->poly_part, nparts, pr->partials, d.scal + 16, d.counters,
+                                 d.stream);
+      db_count_launch(1);
+    }
     if (pr->world > 1) {
       // sum the model polynomials of all ranks, then E0 = x - V0
       db_allreduce(pr, pr->E0, 3 * 8 * d.R);  // E0 | E1 | E2 are contiguous
@@ -126,12 +140,12 @@ static void line_setup(LbfgsCtx *c, const double *xk, const double *pk) {
       db_count_launch(1);
     }
   }
-  if (!c->robust && !db_opt(DB_OPT_LINE_DIRECT)) {
-    // the Gaussian cost along the line is a quartic in alpha: five reductions, then every cost
-    // evaluation of the line search is arithmetic on the host
-    db_launch_line_poly(pr->E0, pr->E1, pr->E2, 4 * d.R, pr->partials, d.scal + 16, d.counters,
-                        d.stream);
-    db_count_launch(1);
+  if (want_poly) {
+    if (!fold_poly) {
+      db_launch_line_poly(pr->E0, pr->E1, pr->E2, 4 * d.R, pr->partials, d.scal + 16, d.counters,
+                          d.stream);
+      db_count_launch(1);
+    }
     DB_CHECK(cudaMemcpyAsync(d.h_scal + 16, d.scal + 16, 5 * sizeof(double), cudaMemcpyDeviceToHost,
                              d.stream));
     db_stream_sync(d.stream);
@@ -155,15 +169,16 @@ static double line_cost(LbfgsCtx *c, double alpha) {
   return db_read_scalar(pr, 0);
 }
 
-// gradient at p (device) into g (device); if from_line, the residual is taken from the line model at
-// alpha instead of a fresh predict
-static void grad_eval(LbfgsCtx *c, const double *p, double *g, bool from_line, double alpha) {
+// gradient at p (device) into g (device) from the residual at p in pr->res: taken from the line
+// model at alpha (RES_LINE), formed by a fresh predict (RES_PREDICT), or already there (RES_HELD)
+enum { RES_PREDICT, RES_LINE, RES_HELD };
+static void grad_eval(LbfgsCtx *c, const double *p, double *g, int res_src, double alpha) {
   dirac_b200_problem *pr = c->pr;
   DevProblem &d = pr->d;
-  if (from_line) {
+  if (res_src == RES_LINE) {
     db_launch_line_residual(pr->E0, pr->E1, pr->E2, pr->res, 4 * d.R, alpha, d.stream);
     db_count_launch(1);
-  } else {
+  } else if (res_src == RES_PREDICT) {
     db_predict_dev(pr, p, pr->res, 1, 0, 0.0, 0);
   }
   db_grad_dev(pr, p, g, c->robust, c->nu);
@@ -320,10 +335,14 @@ struct LbfgsTrace {
   int niter;
 };
 
-// p: m x 1 in/out (host).  robust != 0 -> Student's-t cost with nu.
+// p: m x 1 in/out (host).  robust != 0 -> Student's-t cost with nu.  res_held: pr->res already is
+// the residual x - V(p), so the first gradient needs no predict.
 // Iteration logic of lbfgs_fit_fullbatch (lbfgs.c:479-640); vectors on the device.
-static void lbfgs_run(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
-                      double nu, LbfgsTrace *tr) {
+// Returns the number of accepted steps.  On return pr->res is the residual at the returned p: every
+// accepted step leaves the line residual at the new iterate there, and a loop that ends without a
+// step leaves the one it started from.
+static int lbfgs_run(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
+                      double nu, bool res_held, LbfgsTrace *tr) {
   DevProblem &d = pr->d;
   LbfgsCtx ctx;
   ctx.pr = pr;
@@ -337,7 +356,7 @@ static void lbfgs_run(dirac_b200_problem *pr, double *p, int m, int itmax, int M
     // the alpha_i of one recursion live in the shared memory of k_lbfgs_direction
     fprintf(stderr, "dirac_b200: LBFGS memory size %d exceeds the %d pairs the two-loop recursion "
                     "can hold; the LBFGS stage is skipped\n", M, db_lbfgs_direction_max_pairs());
-    return;
+    return 0;
   }
   // one allocation: xk | xk1 | gk | pk | s[M] | y[M] | rho[M]
   double *ws = (double *)db_malloc(sizeof(double) * ((size_t)m * (4 + 2 * (size_t)M) + M + 8));
@@ -347,7 +366,7 @@ static void lbfgs_run(dirac_b200_problem *pr, double *p, int m, int itmax, int M
   double step, alphak;
   int ck, ci, cm;
   DB_CHECK(cudaMemcpyAsync(xk, p, sizeof(double) * m, cudaMemcpyHostToDevice, d.stream));
-  grad_eval(&ctx, xk, gk, false, 0.0);
+  grad_eval(&ctx, xk, gk, res_held ? RES_HELD : RES_PREDICT, 0.0);
   db_launch_lbfgs_nrm2(gk, m, nrm_dev, d.stream);
   db_count_launch(1);
   double gradnrm = sqrt(db_read_scalar(pr, 24));
@@ -373,7 +392,7 @@ static void lbfgs_run(dirac_b200_problem *pr, double *p, int m, int itmax, int M
     double *sk = s + (size_t)cm;
     double *yk = y + (size_t)cm;
     db_launch_lbfgs_step(xk, pk, gk, xk1, sk, yk, m, alphak, d.stream);
-    grad_eval(&ctx, xk1, gk, true, alphak);
+    grad_eval(&ctx, xk1, gk, RES_LINE, alphak);
     db_launch_lbfgs_update(gk, sk, yk, xk1, xk, m, rho + ci, nrm_dev, d.stream);
     db_count_launch(2);
     gradnrm = sqrt(db_read_scalar(pr, 24));
@@ -397,11 +416,12 @@ static void lbfgs_run(dirac_b200_problem *pr, double *p, int m, int itmax, int M
   DB_CHECK(cudaMemcpyAsync(p, xk, sizeof(double) * m, cudaMemcpyDeviceToHost, d.stream));
   db_stream_sync(d.stream);
   db_free(ws);
+  return (int)ctx.ngrad - 1;  // one gradient at the start, one per accepted step
 }
 
-void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
-                  double nu) {
-  lbfgs_run(pr, p, m, itmax, M, robust, nu, nullptr);
+int db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
+                 double nu, bool res_held) {
+  return lbfgs_run(pr, p, m, itmax, M, robust, nu, res_held, nullptr);
 }
 
 // test hook: the line model of the resident problem along pk from xk (host vectors of npar doubles),
@@ -441,6 +461,25 @@ extern "C" void dirac_b200_line_model(dirac_b200_problem *pr, const double *xk, 
   db_free(dx);
 }
 
+// test hook: the quartic of the line model left by the last dirac_b200_line_model, by the separate
+// pass over E0, E1 and E2 (k_line_poly) that sharded runs take; poly: 5 doubles out (host)
+extern "C" void dirac_b200_line_poly(dirac_b200_problem *pr, double *poly) {
+  DevProblem &d = pr->d;
+  db_launch_line_poly(pr->E0, pr->E1, pr->E2, 4 * d.R, pr->partials, d.scal + 16, d.counters,
+                      d.stream);
+  DB_CHECK(cudaMemcpyAsync(d.h_scal + 16, d.scal + 16, 5 * sizeof(double), cudaMemcpyDeviceToHost,
+                           d.stream));
+  db_stream_sync(d.stream);
+  DB_CHECK(cudaGetLastError());
+  for (int j = 0; j < 5; j++) poly[j] = d.h_scal[16 + j];
+}
+
+// test hook: the residual the resident problem holds (what the solvers left in pr->res), API layout
+extern "C" void dirac_b200_residual(dirac_b200_problem *pr, double *out) {
+  db_download_vis(pr, pr->res, out);
+  DB_CHECK(cudaGetLastError());
+}
+
 // test hook: LBFGS on the resident problem's data from p (host, npar doubles, in/out) as bfgsfit runs
 // it, with the trace of every iteration (LbfgsTrace; arrays of itmax entries, iterates itmax x npar).
 // Returns the number of iterations, or -1 if the memory size M cannot be held.
@@ -450,7 +489,7 @@ extern "C" int dirac_b200_lbfgs_trace(dirac_b200_problem *pr, double *p, int itm
   if ((M < 1 ? 1 : M) > db_lbfgs_direction_max_pairs()) return -1;
   LbfgsTrace tr;
   tr.alphak = alphak; tr.ncost = ncost; tr.slot = slot; tr.gnorm = gnorm; tr.iterates = iterates;
-  lbfgs_run(pr, p, (int)pr->d.npar, itmax, M, robust, nu, &tr);
+  lbfgs_run(pr, p, (int)pr->d.npar, itmax, M, robust, nu, false, &tr);
   return tr.niter;
 }
 

@@ -96,6 +96,9 @@ extern "C" int dirac_b200_set_option(const char *name, int value) {
   if (!strcmp(name, "rtr_nu_unjoined")) { g_opt[DB_OPT_RTR_NU_UNJOINED] = value; return 0; }
   // sagefit_visibilities_admm: LM on the augmented cost instead of the reference's robust RTR
   if (!strcmp(name, "admm_lm")) { g_opt[DB_OPT_ADMM_LM] = value; return 0; }
+  // sagefit: hand back the residual the sweeps kept even when no LBFGS step replaced it (the one
+  // the LBFGS stage starts from), instead of predicting it afresh
+  if (!strcmp(name, "sweep_residual")) { g_opt[DB_OPT_SWEEP_RESIDUAL] = value; return 0; }
   return -1;
 }
 // SMs of the current device (grids of the one-wave kernels are sized from it)
@@ -428,7 +431,7 @@ extern "C" void dirac_b200_destroy(dirac_b200_problem *pr) {
   db_free(pr->partials); db_free(pr->res); db_free(pr->g); db_free(pr->vis_stage);
   if (pr->pm) db_free(pr->pm);
   if (pr->xb) { db_free(pr->xb); db_free(pr->pp_start); }
-  if (pr->E0) db_free(pr->E0);  // E1, E2 live inside E0's allocation
+  if (pr->E0) db_free(pr->E0);  // E1, E2 and poly_part live inside E0's allocation
   cudaFreeHost(d.h_scal);
   free(d.h_clus); free(d.h_chunk_poff);
   if (pr->own_stream) cudaStreamDestroy(d.stream);

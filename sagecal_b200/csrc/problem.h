@@ -101,6 +101,7 @@ struct dirac_b200_problem {
   double *pp_start;       // [npar] Jones at the start of a sharded sweep
   // LBFGS line model (allocated on first use)
   double2 *E0, *E1, *E2;  // [4][R] each
+  double *poly_part;      // [5][db_stream_all_nblocks] per-CTA sums of the line quartic (one GPU)
   struct RtrWork *rtr;    // RTR / NSD solvers (rtr.cu), allocated on first use
 };
 
@@ -194,6 +195,8 @@ extern "C" {
 void db_launch_residual_cost(const double2 *x, const double2 *pm, double2 *out, long long n4,
                              int out_mode, int cost_mode, double inv_nu, double *partials,
                              double *cost, unsigned int *counter, cudaStream_t st);
+void db_launch_sumsq(const double2 *v, long long n4, double *partials, double *out,
+                     unsigned int *counter, cudaStream_t st);
 void db_launch_axpby(const double2 *x, double2 *y, long long n4, double a, double b,
                      cudaStream_t st);
 void db_launch_cluster_rowmap(const double2 *coh_k, const double2 *in, const double2 *in2,

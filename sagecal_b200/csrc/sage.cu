@@ -20,8 +20,8 @@ void db_rlm_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, doubl
                   double *robust_nu, double *info, bool hidden_ready);
 bool db_cluster_needs_rowmap(const dirac_b200_problem *pr, int k);
 void db_cluster_hidden(dirac_b200_problem *pr, int k, double2 *r, int sign, double beta);
-void db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
-                  double nu);
+int db_lbfgs_fit(dirac_b200_problem *pr, double *p, int m, int itmax, int M, int robust,
+                 double nu, bool res_held);
 void db_lbfgs_fit_minibatch(dirac_b200_problem *pr, double *p, int m, int itmax, int M, double nu);
 void db_rtr_chunk(dirac_b200_problem *pr, int k, int ck, double *pblk_dev, double2 *r, int kind,
                   int itmax_a, int itmax_b, double nulow, double nuhigh, double *robust_nu,
@@ -245,21 +245,38 @@ extern "C" int dirac_b200_sagefit(dirac_b200_problem *pr, double *pp, double *x_
   DB_CHECK(cudaMemcpyAsync(pp, d.pp, sizeof(double) * m, cudaMemcpyDeviceToHost, d.stream));
   db_stream_sync(d.stream);
 
+  // Every visit of the sweeps leaves pr->res = x - sum_k model_k at the Jones it hands back (the
+  // sharded merge adds the ranks' changes to it), so the full-batch LBFGS stage starts from that
+  // residual, and each step it accepts leaves the residual at the new iterate in the same place.
+  const bool minibatch = max_lbfgs > 0 && robust && lbfgs_m < 0;
+  const bool lbfgs_stage = max_lbfgs > 0 && (!robust || lbfgs_m != 0);
+  int steps = 0;  // accepted full-batch LBFGS steps
   if (max_lbfgs > 0) {
     if (robust) {
       if (lbfgs_m > 0) {
-        db_lbfgs_fit(pr, pp, m, max_lbfgs, lbfgs_m, 1, robust_nu0);
+        steps = db_lbfgs_fit(pr, pp, m, max_lbfgs, lbfgs_m, 1, robust_nu0, true);
       } else if (lbfgs_m < 0) {
         // stochastic LBFGS over 5 row windows of the interval (lmfit.c:1027-1029)
         db_lbfgs_fit_minibatch(pr, pp, m, max_lbfgs, -lbfgs_m, robust_nu0);
       }
     } else {
-      db_lbfgs_fit(pr, pp, m, max_lbfgs, lbfgs_m, 0, 0.0);
+      steps = db_lbfgs_fit(pr, pp, m, max_lbfgs, lbfgs_m, 0, 0.0, true);
     }
   }
   // final residual, in place in x   (lmfit.c:1039-1044)
-  DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * m, cudaMemcpyHostToDevice, d.stream));
-  db_predict_dev(pr, d.pp, pr->res, 1, 1, 0.0, 0);
+  // (the LBFGS stages move the host Jones only)
+  if (lbfgs_stage)
+    DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * m, cudaMemcpyHostToDevice, d.stream));
+  // After an LBFGS step the residual in pr->res is the line model's at the answer, formed from a
+  // fresh x - V0.  Without one it is the sweeps' (a visit adds and subtracts its cluster's model, and
+  // on a problem solved to rounding level that rounding could show as res_1 > res_0), or, after the
+  // minibatch stage, only some rows' residual: predicted afresh then, as the reference does.
+  if (steps > 0 || (db_opt(DB_OPT_SWEEP_RESIDUAL) && !minibatch)) {
+    db_launch_sumsq(pr->res, 4 * d.R, pr->partials, d.scal, d.counters, d.stream);
+    db_count_launch(1);
+  } else {
+    db_predict_dev(pr, d.pp, pr->res, 1, 1, 0.0, 0);
+  }
   *res_1 = sqrt(db_read_scalar(pr, 0)) / (double)n;
   if (x_out) db_download_vis(pr, pr->res, x_out);
   *mean_nu = robust_nu0;
@@ -312,9 +329,9 @@ int db_bfgsfit_dev(dirac_b200_problem *pr, double *pp, int max_lbfgs, int lbfgs_
   if (max_lbfgs > 0) {
     int M_ = lbfgs_m > 0 ? lbfgs_m : -lbfgs_m;
     if (is_robust_mode(solver_mode)) {
-      db_lbfgs_fit(pr, pp, m, max_lbfgs, M_, 1, mean_nu);
+      db_lbfgs_fit(pr, pp, m, max_lbfgs, M_, 1, mean_nu, false);
     } else {
-      db_lbfgs_fit(pr, pp, m, max_lbfgs, M_, 0, 0.0);
+      db_lbfgs_fit(pr, pp, m, max_lbfgs, M_, 0, 0.0, false);
     }
   }
   DB_CHECK(cudaMemcpyAsync(d.pp, pp, sizeof(double) * m, cudaMemcpyHostToDevice, d.stream));
