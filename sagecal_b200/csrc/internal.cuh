@@ -391,7 +391,7 @@ void db_launch_chol_solve(const double *A, int n, double mu, const double *b, do
 int db_bigtri_available(int n);
 size_t db_bigtri_ws_doubles(int n);
 void db_launch_bigtri_solve(const double *L, int ld, int n, const double *b, double *x, double *ws,
-                            unsigned epoch, int invert, cudaStream_t st);
+                            int *status, cudaStream_t st);
 int db_stream_all_nblocks(int Nbase, int tilesz);
 void db_launch_predict_tma(const StreamAllArgs *a, cudaStream_t st);
 void db_launch_cost_window_tma(const StreamAllArgs *a, cudaStream_t st);

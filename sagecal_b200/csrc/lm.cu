@@ -125,13 +125,7 @@ void db_lm_init(dirac_b200_problem *pr) {
   if (w.own_chol && (size_t)w.lwork < db_chol_ws_doubles(n8)) w.lwork = (int)db_chol_ws_doubles(n8);
   w.cswork = dalloc<double>((size_t)w.lwork);
   w.bc = (!w.own_chol && n8 > 1024) ? db_bigchol_create(n8, BC_BLOCK, BC_INV_PANEL, BC_LOOKAHEAD) : nullptr;
-  w.bt_ws = nullptr;
-  w.bt_epoch = 0;
-  if (!w.own_chol && db_bigtri_available(n8)) {
-    const size_t nd = db_bigtri_ws_doubles(n8);
-    w.bt_ws = dalloc<double>(nd);
-    DB_CHECK(cudaMemsetAsync(w.bt_ws, 0, sizeof(double) * nd, d.stream));  // arrival flags start at 0
-  }
+  w.bt_ws = (!w.own_chol && db_bigtri_available(n8)) ? dalloc<double>(db_bigtri_ws_doubles(n8)) : nullptr;
   w.dbuf = dalloc<double2>((size_t)4 * d.R);
   w.ready = true;
 }
@@ -358,16 +352,18 @@ static int enqueue_solve(dirac_b200_problem *pr, double mu, int linsolv, double 
     db_prof_end(d.stream);
     db_count_launch(1);
   }
-  DB_CHECK(cudaMemcpyAsync(w.Dp, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToDevice, d.stream));
+  // the blocked substitutions read b from J^T e; every other solver works on Dp in place
+  if (linsolv != 0 || !w.bt_ws)
+    DB_CHECK(cudaMemcpyAsync(w.Dp, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToDevice, d.stream));
   db_prof_begin(5, 0.0, d.stream);
   if (linsolv == 0) {
     CS_CHECK(cusolverDnDpotrf(w.cs, CUBLAS_FILL_MODE_LOWER, n, w.JTJ, n, w.cswork, w.lwork,
                               w.devinfo));
     if (w.bt_ws) {
-      // the two substitutions by the blocked dataflow kernels (cusolverDnDpotrs: 0.68 ms at n = 4096)
-      DB_CHECK(cudaMemsetAsync(w.devinfo + 1, 0, sizeof(int), d.stream));
-      db_launch_bigtri_solve(w.JTJ, n, n, w.JTe, w.Dp, w.bt_ws, ++w.bt_epoch, 1, d.stream);
-      db_count_launch(4);
+      // the two substitutions by the blocked dataflow kernels (cusolverDnDpotrs: 0.68 ms at n = 4096);
+      // their prologue clears the status word dpotrs would set
+      db_launch_bigtri_solve(w.JTJ, n, n, w.JTe, w.Dp, w.bt_ws, w.devinfo + 1, d.stream);
+      db_count_launch(2);
     } else {
       CS_CHECK(cusolverDnDpotrs(w.cs, CUBLAS_FILL_MODE_LOWER, n, 1, w.JTJ, n, w.Dp, n,
                                 w.devinfo + 1));
@@ -893,17 +889,17 @@ static void lm_core(dirac_b200_problem *pr, int k, int ck, int t0, int t1, doubl
             db_launch_tri_solve_ld(w.LB + (size_t)slot * w.lb_stride, w.lb_ld, n, w.JTe, w.Dp,
                                    d.stream);
             w.step_fused = w.step_armed;
+          } else if (w.bt_ws) {
+            // no status of its own either
+            skip_info = true;
+            db_launch_bigtri_solve(w.LB + (size_t)slot * w.lb_stride, n, n, w.JTe, w.Dp, w.bt_ws,
+                                   nullptr, d.stream);
           } else {
             DB_CHECK(cudaMemsetAsync(w.devinfo, 0, 2 * sizeof(int), d.stream));
-            if (w.bt_ws) {
-              db_launch_bigtri_solve(w.LB + (size_t)slot * w.lb_stride, n, n, w.JTe, w.Dp, w.bt_ws,
-                                     ++w.bt_epoch, 1, d.stream);
-            } else {
-              DB_CHECK(cudaMemcpyAsync(w.Dp, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToDevice,
-                                       d.stream));
-              CS_CHECK(cusolverDnDpotrs(w.cs, CUBLAS_FILL_MODE_LOWER, n, 1,
-                                        w.LB + (size_t)slot * w.lb_stride, n, w.Dp, n, w.devinfo + 1));
-            }
+            DB_CHECK(cudaMemcpyAsync(w.Dp, w.JTe, sizeof(double) * n, cudaMemcpyDeviceToDevice,
+                                     d.stream));
+            CS_CHECK(cusolverDnDpotrs(w.cs, CUBLAS_FILL_MODE_LOWER, n, 1,
+                                      w.LB + (size_t)slot * w.lb_stride, n, w.Dp, n, w.devinfo + 1));
           }
           db_prof_end(d.stream);
           db_count_launch(1);

@@ -38,7 +38,6 @@ struct LMWork {
   int lwork;
   bool own_chol;  // damped solves by the cluster Cholesky kernel (else cuSOLVER)
   double *bt_ws;  // large systems: workspace of the blocked triangular solves (kernels_bigtri.cu)
-  unsigned bt_epoch;
   BigChol *bc;    // large systems: blocked factorisation of the sweep's batch (bigchol.cu)
   double *jte_part;       // per-CTA station sums of the linear-mapped gradient pass
   bool step_armed, step_fused;  // trial point formed by the solver kernel's epilogue
