@@ -538,4 +538,6 @@ int dirac_b200_bigtri_solve(int n, const double *L, const double *b, double *x, 
 #include "dirac_b200_stochastic.h"
 /* federated stochastic calibration (the projectback manifold average and the slave's ADMM step) */
 #include "dirac_b200_federated.h"
+/* influence-function diagnostics (calculate_diagnostics_gpu, driver option -i 1) */
+#include "dirac_b200_diagnostics.h"
 #endif

@@ -8,6 +8,7 @@
 #include "../../include/dirac_b200_channels.h"
 #include "../../include/dirac_b200_stochastic.h"
 #include "coh.h"
+#include "influence.h"
 #include "problem.h"
 
 // the sky of M clusters, u, v, w of R rows and Nchan channel frequencies on the device through ds, and
@@ -107,16 +108,6 @@ static void upload_row_stations(DeviceScope &ds, const baseline_t *barr, long lo
 
 
 // ---- station beams (precalculate_coherencies_withbeam & co, predict_withbeam.c) -----------------------
-struct BeamSpec {
-  int bf_type;
-  double b_ra0, b_dec0, ph_ra0, ph_dec0, ph_freq0;
-  const double *longitude, *latitude, *time_utc;
-  int tilesz;
-  const int *Nelem;
-  double **xx, **yy, **zz;
-  const elementcoeff *ecoeff;
-  int doBeam;
-};
 // doBeam: Dirac_common.h:120-151
 static bool beam_wide(int doBeam) {
   return doBeam == DOBEAM_ARRAY_WB || doBeam == DOBEAM_FULL_WB || doBeam == DOBEAM_ELEMENT_WB;
@@ -613,17 +604,19 @@ static void correction_inverse(const double *p, const clus_source_t &c, int N, d
 // that cluster's inverse Jones (J + rho I)^-1; phase_only != 0: by the inverse of the phases of its
 // jointly diagonalised solutions (extract_phases, manifold_average.c:399-610).  Rows are predicted
 // whatever their flag.
-static int residuals_multifreq_impl(double *u, double *v, double *w, double *p, double *x, int N,
-                                    int Nbase, int tilesz, baseline_t *barr, clus_source_t *carr,
-                                    int M, double *freqs, int Nchan, double fdelta,
-                                    const std::vector<signed char> &coef, bool clear_x, int ccid,
-                                    double rho, int phase_only, const BeamSpec *beam) {
-  DeviceScope ds;
+// residuals_stage: the same up to the launch, the result left in a.xout on the device (pinv holds
+// the host copy of the correction until the caller's next wait; correct false: no correction)
+static CohArgs residuals_stage(DeviceScope &ds, const double *u, const double *v, const double *w,
+                               const double *p, const double *x, int N, int Nbase, int tilesz,
+                               const baseline_t *barr, const clus_source_t *carr, int M,
+                               const double *freqs, int Nchan, double fdelta,
+                               const std::vector<signed char> &coef, bool clear_x, bool correct,
+                               int ccid, double rho, int phase_only, const BeamSpec *beam,
+                               std::vector<double> &pinv) {
   const long long R = (long long)Nbase * tilesz;
   CohArgs a = stage_sky(ds, carr, M, u, v, w, R, freqs, Nchan, fdelta / (double)Nchan);
   const ResidualTables tb = residual_tables(ds, barr, carr, N, M, coef, ccid, &a);
-  const int cm = tb.cm;
-  std::vector<double> pinv;
+  const int cm = correct ? tb.cm : -1;
   if (cm >= 0) correction_inverse(p, carr[cm], N, rho, phase_only, pinv);
   a.p = ds.upload(p, tb.npar);
   a.pinv = cm >= 0 ? ds.upload(pinv) : nullptr;
@@ -640,8 +633,52 @@ static int residuals_multifreq_impl(double *u, double *v, double *w, double *p, 
   db_launch_residual_multifreq(&a, ds.st);
   db_prof_end(ds.st);
   db_count_launch(1);
+  return a;
+}
+static int residuals_multifreq_impl(double *u, double *v, double *w, double *p, double *x, int N,
+                                    int Nbase, int tilesz, baseline_t *barr, clus_source_t *carr,
+                                    int M, double *freqs, int Nchan, double fdelta,
+                                    const std::vector<signed char> &coef, bool clear_x, int ccid,
+                                    double rho, int phase_only, const BeamSpec *beam) {
+  DeviceScope ds;
+  std::vector<double> pinv;
+  CohArgs a = residuals_stage(ds, u, v, w, p, x, N, Nbase, tilesz, barr, carr, M, freqs, Nchan, fdelta,
+                              coef, clear_x, true, ccid, rho, phase_only, beam, pinv);
+  const size_t nx = (size_t)Nchan * Nbase * tilesz * 4;
   DB_CHECK(cudaMemcpyAsync(x, a.xout, sizeof(double2) * nx, cudaMemcpyDeviceToHost, ds.st));
   ds.sync();
+  return 0;
+}
+
+// Step 1 of calculate_diagnostics_gpu (diagnostics_host.cu): x[chan][row][4] on the device minus the
+// model of every cluster, whatever its id, without correction (diagnostics.c:243-246), and the
+// coherencies of every cluster at channel 0, [M][R][4], by the multi-channel prediction one cluster
+// at a time: the same fluxes (spectral indices included), smearing width and beams as the model
+int db_diagnostics_model(DeviceScope &ds, const double *u, const double *v, const double *w,
+                         const double *p, const double *x, int N, int Nbase, int tilesz,
+                         const baseline_t *barr, const clus_source_t *carr, int M,
+                         const double *freqs, int Nchan, double fdelta, const BeamSpec *beam,
+                         DiagModel *out) {
+  std::vector<double> pinv;
+  const std::vector<signed char> coef(M, -1);
+  const CohArgs r = residuals_stage(ds, u, v, w, p, x, N, Nbase, tilesz, barr, carr, M, freqs, Nchan,
+                                    fdelta, coef, false, false, 0, 0.0, 0, beam, pinv);
+  const long long R = (long long)Nbase * tilesz;
+  CohArgs a = stage_sky(ds, carr, M, u, v, w, R, freqs, 1, fdelta / (double)Nchan);
+  beam_prepare(ds, beam, N, Nbase, barr, &a);
+  double2 *coh = ds.alloc<double2>((size_t)M * 4 * R);
+  DB_CHECK(cudaMemsetAsync(coh, 0, sizeof(double2) * M * 4 * R, ds.st));
+  int seg0 = 0;
+  for (int k = 0; k < M; k++) {  // stage_sky's segments of cluster k (at least one)
+    const int nseg = carr[k].N > COH_SEG_MAX ? (carr[k].N + COH_SEG_MAX - 1) / COH_SEG_MAX : 1;
+    CohArgs ak = a;
+    ak.segs = a.segs + seg0; ak.nseg = nseg; ak.xout = coh + (size_t)k * 4 * R;
+    db_launch_predict_multifreq(&ak, ds.st);
+    seg0 += nseg;
+  }
+  db_count_launch(M);
+  out->x = r.xout; out->coh = coh; out->p = r.p; out->clus_nchunk = r.clus_nchunk;
+  out->clus_chunk0 = r.clus_chunk0; out->chunk_poff = r.chunk_poff;
   return 0;
 }
 // the residual subtracts the clusters with id >= 0 (residual.c:704)
@@ -913,7 +950,7 @@ static bool bands_refused(const char *fn, int nsolbw, int Nchan) {
 
 // the beam arguments of the _withbeam interval calls, checked before any device work: -1 with a
 // message (the reference-named _withbeam calls exit instead)
-static bool beam_refused(const char *fn, const BeamSpec &b, int N, int Nchan) {
+bool beam_refused(const char *fn, const BeamSpec &b, int N, int Nchan) {
   if (b.doBeam == DOBEAM_NONE) return false;
   if (b.doBeam < DOBEAM_NONE || b.doBeam > DOBEAM_ELEMENT_WB) {
     fprintf(stderr, "%s: doBeam = %d is not a beam mode this call takes (0..6; the lunar element "

@@ -36,8 +36,9 @@ static cudaEvent_t prof_event() {
 }
 // kinds: 13 k_stream_band (band cost or residual), 14 k_grad_tma_band (band gradient), 15
 // k_beam_tables (station beam tables), 16 the stochastic interval's coherency predictions, 17
-// k_manifold_projectback
-#define DB_PROF_KINDS 18
+// k_manifold_projectback; calculate_diagnostics_gpu: 18 the model stage, 19 Hessians and right-hand
+// sides, 20 the LU solves, 21 k_infl_dr, 22 the four eigenvalue problems, 23 the whole call
+#define DB_PROF_KINDS 24
 static unsigned long long g_kind_count[DB_PROF_KINDS] = {0};
 extern "C" unsigned long long dirac_b200_kernel_count(int kind) {
   return (kind >= 0 && kind < DB_PROF_KINDS) ? g_kind_count[kind] : 0ull;
@@ -52,6 +53,19 @@ void db_prof_begin(int kind, double bytes, cudaStream_t st) {
 void db_prof_end(cudaStream_t st) {
   if (!g_prof_on) return;
   DB_CHECK(cudaEventRecord(g_prof.back().b, st));
+}
+// a timed span that may enclose other timed launches: db_prof_open returns its record (-1 when
+// profiling is off), db_prof_close ends that record rather than the last one
+int db_prof_open(int kind, double bytes, cudaStream_t st) {
+  if (!g_prof_on) {
+    if (kind >= 0 && kind < DB_PROF_KINDS) g_kind_count[kind]++;
+    return -1;
+  }
+  db_prof_begin(kind, bytes, st);
+  return (int)g_prof.size() - 1;
+}
+void db_prof_close(int rec, cudaStream_t st) {
+  if (rec >= 0 && g_prof_on && rec < (int)g_prof.size()) DB_CHECK(cudaEventRecord(g_prof[rec].b, st));
 }
 extern "C" void dirac_b200_profile_enable(int on) {
   for (auto &r : g_prof) { g_evpool.push_back(r.a); g_evpool.push_back(r.b); }

@@ -154,6 +154,9 @@ void db_download_coh(const double2 *coh, double *x, int M, long long R, cudaStre
 void db_count_launch(int n);
 void db_prof_begin(int kind, double bytes, cudaStream_t st);
 void db_prof_end(cudaStream_t st);
+// a timed span enclosing other timed launches (db_prof_close ends its own record)
+int db_prof_open(int kind, double bytes, cudaStream_t st);
+void db_prof_close(int rec, cudaStream_t st);
 cudaStream_t db_new_stream(int *owned);
 void db_upload_vis(dirac_b200_problem *pr, const double *h, double2 *dst);
 void db_download_vis(dirac_b200_problem *pr, const double2 *src, double *h);

@@ -62,6 +62,9 @@ STOCHASTIC_EXPORTED = ["dirac_b200_stochastic_interval", "dirac_b200_stochastic_
 FEDERATED_EXPORTED = ["dirac_b200_stochastic_federated_interval", "calculate_manifold_average_projectback", "dirac_b200_manifold_projectback_dev",
                       "dirac_b200_consensus_prod_inverse_fed", "dirac_b200_federated_bands_update"]
 
+#: every symbol include/dirac_b200_diagnostics.h declares (influence-function diagnostics, -i 1)
+DIAGNOSTICS_EXPORTED = ["calculate_diagnostics_gpu"]
+
 
 class DiracB200(DiracAPI):
     """The product library: the reference entry points (inherited bindings) plus the thin
@@ -126,6 +129,53 @@ class DiracB200(DiracAPI):
         n, b = C.c_ulonglong(0), C.c_ulonglong(0)
         self.lib.dirac_b200_transfer_stats(C.byref(n), C.byref(b), 1 if reset else 0)
         return n.value, b.value
+
+    def calculate_diagnostics_gpu(self, u, v, w, p, x, N, Nbase, tilesz, barr, sky, freqs, fdelta,
+                                  beam=None, rho=None, Bpoly=None, Bi=None, Npoly=0, tdelta=10.0,
+                                  dec0=1.0, Nt=4):
+        """influence-function diagnostics (Dirac_radio.h:676).  x[chan][row][8]: data in; out: the
+        eigenvalues of the four dR correlations in channel 0 of every timeslot, the residual in the
+        other channels.  beam: a BeamSetup or None; rho [M], Bpoly [Npoly], Bi [M][Npoly][Npoly]: the
+        consensus term (all three or none)"""
+        L = self.lib
+        d = C.c_double
+        L.calculate_diagnostics_gpu.restype = C.c_int
+        freqs = np.ascontiguousarray(freqs, dtype=np.float64)
+        f64 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float64)
+        rho, Bpoly, Bi = f64(rho), f64(Bpoly), f64(Bi)
+        opt = lambda a: None if a is None else dptr(a)
+        if beam is None:
+            bhead = (0, d(0.0), d(0.0), d(0.0), d(0.0), d(0.0), None, None, None)
+            btail = (None, None, None, None, None, 0)
+        else:
+            bhead, btail = beam.head(), beam.tail()
+        return L.calculate_diagnostics_gpu(
+            dptr(u), dptr(v), dptr(w), dptr(p), dptr(x), N, Nbase, tilesz, barr, sky.arr, sky.M,
+            dptr(freqs), len(freqs), d(fdelta), d(tdelta), d(dec0), *bhead, *btail, opt(rho), opt(Bpoly),
+            opt(Bi), sky.M, Npoly, len(freqs), Nt)
+
+    def diagnostics_eval(self, N, Nbase, tilesz, barr, p, nchunk, coh, res, X):
+        """the influence kernels of one cluster (dirac_b200_diagnostics_eval): coh, res [R][4] complex
+        (channel 0), p [nchunk][N][8], X [4N][Nbase] complex.  returns (H [4N][4N] before the
+        conditioning, AdV [4N][Nbase], dR [4][Nbase][Nbase], each complex), or None where refused"""
+        L = self.lib
+        L.dirac_b200_diagnostics_eval.restype = C.c_int
+        L.dirac_b200_diagnostics_eval.argtypes = ([C.c_int] * 3 + [C.POINTER(baseline_t), c_double_p,
+                                                   C.c_int] + [c_double_p] * 6)
+        cf = lambda a: np.ascontiguousarray(a, dtype=np.complex128)
+        n4 = 4 * N
+        H = np.zeros((n4, n4), dtype=np.complex128, order="F")
+        A = np.zeros((n4, Nbase), dtype=np.complex128, order="F")
+        dR = np.zeros((4, Nbase, Nbase), dtype=np.complex128)
+        Xf = np.asfortranarray(X, dtype=np.complex128)
+        p = np.ascontiguousarray(p, dtype=np.float64)
+        vp = lambda a: a.ctypes.data_as(c_double_p)
+        rv = L.dirac_b200_diagnostics_eval(N, Nbase, tilesz, barr, dptr(p), nchunk, vp(cf(coh)),
+                                           vp(cf(res)), vp(Xf), vp(H), vp(A), vp(dR))
+        if rv != 0:
+            return None
+        # dR[c] is column major: element (row b, column bl) at bl*Nbase + b
+        return H, A, np.ascontiguousarray(dR.transpose(0, 2, 1))
 
     def noise_decisions(self, reset=False) -> int:
         self.lib.dirac_b200_noise_decisions.restype = C.c_long
