@@ -540,4 +540,6 @@ int dirac_b200_bigtri_solve(int n, const double *L, const double *b, double *x, 
 #include "dirac_b200_federated.h"
 /* influence-function diagnostics (calculate_diagnostics_gpu, driver option -i 1) */
 #include "dirac_b200_diagnostics.h"
+/* full-batch calibration of one tile (coherencies, SAGE fit and residual in one call) */
+#include "dirac_b200_fullbatch.h"
 #endif

@@ -9,15 +9,22 @@
 #ifndef DIRAC_B200_FEDERATED_H
 #define DIRAC_B200_FEDERATED_H
 
+#ifdef __cplusplus
+extern "C" {
+#endif
+/* sum `count` doubles at device address `dev` over all ranks, in place, enqueued on the cudaStream_t
+ * `stream` (the same contract as the callback of dirac_b200_set_comm).  Declared before the include
+ * below: dirac_b200_fullbatch.h, which dirac_b200.h includes, takes it too. */
+typedef void (*dirac_b200_allreduce_fn)(void *dev, long long count, void *stream, void *user);
+#ifdef __cplusplus
+}
+#endif
+
 #include "dirac_b200.h"
 
 #ifdef __cplusplus
 extern "C" {
 #endif
-
-/* sum `count` doubles at device address `dev` over all ranks, in place, enqueued on the cudaStream_t
- * `stream` (the same contract as the callback of dirac_b200_set_comm) */
-typedef void (*dirac_b200_allreduce_fn)(void *dev, long long count, void *stream, void *user);
 
 /* replaces the stochastic slave's interval (sagecal_stochastic_slave.cpp:650-881) and, for it, the
  * master's exchange (sagecal_stochastic_master.cpp:334-354), for one measurement set on this rank, no

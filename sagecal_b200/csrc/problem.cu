@@ -37,8 +37,9 @@ static cudaEvent_t prof_event() {
 // kinds: 13 k_stream_band (band cost or residual), 14 k_grad_tma_band (band gradient), 15
 // k_beam_tables (station beam tables), 16 the stochastic interval's coherency predictions, 17
 // k_manifold_projectback; calculate_diagnostics_gpu: 18 the model stage, 19 Hessians and right-hand
-// sides, 20 the LU solves, 21 k_infl_dr, 22 the four eigenvalue problems, 23 the whole call
-#define DB_PROF_KINDS 24
+// sides, 20 the LU solves, 21 k_infl_dr, 22 the four eigenvalue problems, 23 the whole call;
+// dirac_b200_fullbatch_tile: 24 the coherencies at freq0 (beam tables included), 25 the SAGE fit
+#define DB_PROF_KINDS 26
 static unsigned long long g_kind_count[DB_PROF_KINDS] = {0};
 extern "C" unsigned long long dirac_b200_kernel_count(int kind) {
   return (kind >= 0 && kind < DB_PROF_KINDS) ? g_kind_count[kind] : 0ull;
@@ -173,6 +174,7 @@ static void cache_release_all() {
   g_cached_bytes = 0;
 }
 extern "C" void dirac_b200_release_cache(void) { cache_release_all(); }
+size_t db_cached_bytes() { return g_cached_bytes; }
 void *db_malloc(size_t bytes) {
   bytes = (bytes + 255) & ~(size_t)255;
   auto it = g_free_blocks.find(bytes);

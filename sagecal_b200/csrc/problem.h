@@ -111,6 +111,8 @@ void db_flag_wait(const volatile unsigned long long *flag, unsigned long long ep
                   cudaStream_t st);
 void *db_malloc(size_t bytes);
 void db_free(void *p);
+// device memory freed blocks hold in the allocator's cache (a failed cudaMalloc gives it back)
+size_t db_cached_bytes();
 // exits with a message if there is no CUDA device: this library has no CPU fallback
 void require_gpu();
 

@@ -8,6 +8,7 @@ import os
 import numpy as np
 
 from .dirac_api import DiracAPI, SkyModel, baseline_t, clus_source_t, c_double_p, dptr, cptr  # noqa: F401
+from .dirac_api import c_int_p, elementcoeff
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdirac_b200.so")
@@ -64,6 +65,9 @@ FEDERATED_EXPORTED = ["dirac_b200_stochastic_federated_interval", "calculate_man
 
 #: every symbol include/dirac_b200_diagnostics.h declares (influence-function diagnostics, -i 1)
 DIAGNOSTICS_EXPORTED = ["calculate_diagnostics_gpu"]
+
+#: every symbol include/dirac_b200_fullbatch.h declares (full-batch calibration of one tile)
+FULLBATCH_EXPORTED = ["dirac_b200_fullbatch_tile", "dirac_b200_fullbatch_tile_withbeam"]
 
 
 class DiracB200(DiracAPI):
@@ -176,6 +180,44 @@ class DiracB200(DiracAPI):
             return None
         # dR[c] is column major: element (row b, column bl) at bl*Nbase + b
         return H, A, np.ascontiguousarray(dR.transpose(0, 2, 1))
+
+    def fullbatch_tile(self, u, v, w, x, xo, N, Nbase, tilesz, barr, sky, freq0, deltaf, freqs, pp,
+                       uvmin=0.0, uvmax=1e9, max_emiter=3, max_iter=2, max_lbfgs=10, lbfgs_m=7,
+                       linsolv=0, solver_mode=1, nulow=2.0, nuhigh=30.0, randomize=0, do_chan=0,
+                       ccid=-99999, rho=1e-9, phase_only=0, rank=0, world=1, allreduce=None,
+                       beam=None):
+        """dirac_b200_fullbatch_tile (beam: a BeamSetup, through the _withbeam variant): one tile of
+        the full-batch driver in one call.  x [row][8] data -> the fit's residual, xo [Nchan][row][8]
+        data -> residual, pp start -> solution, barr flags, all in place; allreduce: a ctypes callback
+        of sagecal_b200.dist.make_allreduce, or None for the library's NCCL communicator.
+        returns (retval, mean_nu, res_0, res_1, res_00 [Nchan], res_01 [Nchan])"""
+        L = self.lib
+        dp, i, d = c_double_p, C.c_int, C.c_double
+        for a in (u, v, w, x, xo, pp):
+            assert a.dtype == np.float64 and a.flags.c_contiguous
+        freqs = np.ascontiguousarray(freqs, dtype=np.float64)
+        head_t = [dp] * 5 + [i] * 3 + [C.POINTER(baseline_t), C.POINTER(clus_source_t), i, i, d, d, dp, i,
+                                       d, d]
+        tail_t = [dp] + [i] * 6 + [d, d] + [i] * 3 + [d] + [i] * 3 + [C.c_void_p] * 2 + [dp] * 5
+        if beam is None:
+            fn, bargs = L.dirac_b200_fullbatch_tile, ()
+            fn.argtypes = head_t + tail_t
+        else:
+            dpp = C.POINTER(c_double_p)
+            fn, bargs = L.dirac_b200_fullbatch_tile_withbeam, (*beam.head(), *beam.tail())
+            fn.argtypes = head_t + [i] + [d] * 5 + [dp] * 3 + [c_int_p, dpp, dpp, dpp,
+                                                               C.POINTER(elementcoeff), i] + tail_t
+        fn.restype = i
+        nchan = len(freqs)
+        nu, r0, r1 = C.c_double(0.0), C.c_double(0.0), C.c_double(0.0)
+        r00, r01 = np.zeros(nchan), np.zeros(nchan)
+        cb = C.cast(allreduce, C.c_void_p) if allreduce is not None else None
+        rv = fn(dptr(u), dptr(v), dptr(w), dptr(x), dptr(xo), N, Nbase, tilesz, barr, sky.arr, sky.M,
+                sky.Mt, freq0, deltaf, dptr(freqs), nchan, uvmin, uvmax, *bargs, dptr(pp), max_emiter,
+                max_iter, max_lbfgs, lbfgs_m, linsolv, solver_mode, nulow, nuhigh, randomize, do_chan,
+                ccid, rho, phase_only, rank, world, cb, None, C.byref(nu), C.byref(r0), C.byref(r1),
+                dptr(r00), dptr(r01))
+        return rv, nu.value, r0.value, r1.value, r00, r01
 
     def noise_decisions(self, reset=False) -> int:
         self.lib.dirac_b200_noise_decisions.restype = C.c_long
