@@ -1,15 +1,15 @@
 """CPU: the plain references the GPU tests of the line model, the RTR evaluator, the IRLS update, the
-LBFGS two-loop recursion, the segmented sky staging, the minibatch band passes and the LM cluster
-passes lean on, pinned
+LBFGS two-loop recursion, the segmented sky staging, the minibatch band passes, the LM cluster
+passes and the full-interval passes lean on, pinned
 against the restatement (oracle/liboracle.so) or the compiled reference's recorded answers before a GPU
 is involved."""
 import numpy as np
 import pytest
 
 import orcdirac
-from util import (BAND_CASES, BAND_FAULTS, CP_FAULTS, CP_RUNS, U64, band_case, band_consensus, band_ref,
-                  big_cluster_sky, chunk_offset, chunk_tiles, cluster_case, cluster_pass_ref, cp_ref_args,
-                  cp_run_applies,
+from util import (BAND_CASES, BAND_FAULTS, CP_FAULTS, CP_RUNS, INTERVAL_FAULTS, U64, band_case,
+                  band_consensus, band_ref, big_cluster_sky, chunk_offset, chunk_tiles, cluster_case,
+                  cluster_pass_ref, cp_ref_args, cp_run_applies, interval_case, interval_ref,
                   cluster_rowmap_ref, irls_ref, lbfgs_pairs, line_model_ref, maps_agree,
                   mult_hessian_ref, relerr, rtr_eval_ref, rtr_weights_ref, small_problem,
                   split_cluster)
@@ -419,5 +419,100 @@ def test_cluster_pass_cases_discriminate():
                 worst = max(worst, _worst(np.abs(bad["out"] - good["out"]), good["out_bound"]),
                             _worst(abs(bad["cost"] - good["cost"]), good["cost_bound"]),
                             _worst(np.abs(bad["jte"] - good["jte"]), good["jte_bound"]))
+        print("fault %s: largest error / bound %.3g" % (fault, worst))
+        assert worst > 1e3, (fault, worst)
+
+
+# ---- the full-interval passes: util.interval_ref ----------------------------------------------------------
+@pytest.mark.parametrize("nu", [None, 2.0, 30.0], ids=["gaussian", "nu2", "nu30"])
+def test_interval_reference_matches_compiled_reference(ref, nu):
+    """util.interval_ref against the compiled reference (minimize_viz_full_pth, cost_func /
+    robust_cost_func, grad_func / robust_grad_func) and the oracle's restatement of them, on an
+    interval with non-zero data on flag-1 and uv-cut rows and a hybrid cluster whose row and timeslot
+    chunk maps disagree (n9: nchunk 2 over 5 timeslots), near and far from the truth"""
+    from sagecal_b200.dirac_api import SkyModel, make_barr
+    case = interval_case("n9")
+    pr = case["pr"]
+    assert not maps_agree(case["tilesz"], case["Nbase"], case["nchunk"])
+    barr, sky = make_barr(pr.sta1, pr.sta2, pr.flag), SkyModel(pr.clusters, pr.N)
+    md = ref.me_data(pr.N, pr.Nbase, pr.tilesz, barr, sky, pr.coh, robust_nu=2.0 if nu is None else nu)
+    orc = orcdirac.Oracle(pr) if orcdirac.available() else None
+    robust = nu is not None
+    worst = dict(model=0.0, cost=0.0, grad=0.0)
+    for s in ("A", "B"):
+        p = case["points"][s]
+        r = interval_ref(case, p, (nu,))
+        q = r["passes"][nu]
+        # the reference's cost is one more rounding away (the square of dnrm2, or the threads' sums)
+        cost_bound = q["cost_bound"] + 4 * U64 * abs(q["cost"])
+        want = [(ref.predict_full(p.copy(), md, 8 * pr.Nbase1), ref.cost(p.copy(), pr.x, md, robust),
+                 ref.grad(p.copy(), pr.x, md, robust))]
+        if orc is not None:
+            want.append((orc.predict_full(p), orc.cost(p, pr.x, robust, 2.0 if nu is None else nu),
+                         orc.grad(p, pr.x, robust, 2.0 if nu is None else nu)))
+        for V, c, g in want:
+            err = np.abs(V - r["model"])
+            assert (err <= r["res_bound"]).all(), (s, _worst(err, r["res_bound"]))
+            worst["model"] = max(worst["model"], _worst(err, r["res_bound"]))
+            assert abs(c - q["cost"]) <= cost_bound, (s, c, q["cost"], cost_bound)
+            worst["cost"] = max(worst["cost"], abs(c - q["cost"]) / cost_bound)
+            err = np.abs(g - q["grad"])
+            assert (err <= q["grad_bound"]).all(), (s, _worst(err, q["grad_bound"]))
+            worst["grad"] = max(worst["grad"], _worst(err, q["grad_bound"]))
+        # a real error would be far above the bound
+        assert np.abs(q["grad"]).max() > 1e6 * q["grad_bound"].max()
+    print("interval_ref vs compiled reference (nu %s): largest error / bound: model %.3g, cost %.3g, "
+          "gradient %.3g" % (nu, worst["model"], worst["cost"], worst["grad"]))
+
+
+@pytest.mark.parametrize("nu", [None, 5.0], ids=["gaussian", "student-t"])
+def test_interval_reference_gradient_is_the_derivative_of_its_cost(nu):
+    """calculus, no other code: on an interval whose hybrid chunks are the same under the model's row
+    map and the gradient's timeslot map (n33h3), the fourth-order central difference of the cost along
+    a direction confined to one chunk block is -grad . d for the Gaussian gradient (the reference's
+    grad_func returns minus the true gradient) and +grad . d for the Student's-t one"""
+    case = interval_case("n33h3")
+    assert maps_agree(case["tilesz"], case["Nbase"], case["nchunk"])
+    N = case["N"]
+    rng = np.random.default_rng(4)
+    p = case["points"]["B"]
+    q = interval_ref(case, p, (nu,))["passes"][nu]
+    sign = -1.0 if nu is None else 1.0
+    h = 1e-4
+    worst = 0.0
+    for ci in range(case["Mt"]):
+        d = np.zeros(case["m"])
+        d[8 * N * ci:8 * N * (ci + 1)] = rng.normal(0, 1, 8 * N)
+        f = [interval_ref(case, p + t * h * d, (nu,))["passes"][nu]["cost"] for t in (-2, -1, 1, 2)]
+        fd = (f[0] - 8 * f[1] + 8 * f[2] - f[3]) / (12 * h)
+        want = sign * np.dot(q["grad"], d)
+        off = abs(fd - want) / np.dot(np.abs(q["grad"]) + q["grad_bound"], np.abs(d))
+        worst = max(worst, off)
+        assert off < 1e-7, (ci, fd, want)
+    print("interval_ref gradient vs central differences (nu %s): largest relative deviation %.3g"
+          % (nu, worst))
+
+
+def test_interval_cases_discriminate():
+    """every deliberate fault of INTERVAL_FAULTS, applied to interval_ref, moves some quantity of some
+    GPU case (test_gpu_interval_passes.py) past its bound by more than 10^3: the cases can see it"""
+    names = ["n2", "n9", "n33h3", "n33h4", "n40m1", "n40m2", "n40m4", "all-flagged"]
+    nus = (None, 2.0, 30.0)
+    runs = []
+    for n in names:
+        case = interval_case(n)
+        for s in ("A", "B"):
+            p = case["points"][s]
+            runs.append((case, p, interval_ref(case, p, nus)))
+    for fault in INTERVAL_FAULTS:
+        worst = 0.0
+        for case, p, good in runs:
+            bad = interval_ref(case, p, nus, fault=fault)
+            worst = max(worst, _worst(np.abs(bad["res"] - good["res"]), good["res_bound"]),
+                        _worst(np.abs(bad["model"] - good["model"]), good["res_bound"]))
+            for nu in nus:
+                g, b = good["passes"][nu], bad["passes"][nu]
+                worst = max(worst, _worst(abs(b["cost"] - g["cost"]), g["cost_bound"]),
+                            _worst(np.abs(b["grad"] - g["grad"]), g["grad_bound"]))
         print("fault %s: largest error / bound %.3g" % (fault, worst))
         assert worst > 1e3, (fault, worst)

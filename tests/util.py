@@ -1104,3 +1104,228 @@ def cp_expected_kernel(case, k, ck, kw):
     if kw["mode"] == 4 or kw.get("wt") or not fits:
         return "split"
     return "lin_grad"
+
+
+# ---- the full-interval passes (k_stream_all<0>, k_grad_tma_split) ---------------------------------------
+#: (N, M, timeslots, nchunk of the clusters) of the full-interval cases (tests/test_gpu_interval_passes.py)
+INTERVAL_CASES = {
+    "n2": (2, 1, 1, [1]),
+    "n9": (9, 3, 5, [1, 2, 1]),
+    "n33h3": (33, 7, 9, [1, 3, 1, 1, 3, 1, 1]),
+    "n33h4": (33, 7, 9, [1, 4, 1, 1, 4, 1, 1]),
+    "n40m1": (40, 1, 3, [1]),
+    "n40m2": (40, 2, 3, [1, 1]),
+    "n40m4": (40, 4, 3, [1, 1, 1, 1]),
+    "n62": (62, 64, 11, [2 if k % 8 == 3 else (3 if k == 60 else 1) for k in range(64)]),
+    "n62t120": (62, 8, 120, [1, 1, 1, 1, 1, 3, 1, 1]),
+    "n512": (512, 32, 5, [2 if k == 20 else 1 for k in range(32)]),
+    "n520": (520, 4, 2, [1, 1, 1, 1]),
+    "all-flagged": (9, 3, 5, [1, 2, 1]),
+}
+
+#: deliberate faults interval_ref can apply to itself (tests/test_cpu_refs.py: sensitivity of the cases)
+INTERVAL_FAULTS = ("grad_over_flagged", "grad_row_map", "robust_weight_complex",
+                   "drop_last_timeslot_block", "drop_last_q_tile", "drop_last_p_of_tile",
+                   "stale_ring_stage", "drop_third_warp", "grad_sign")
+
+
+def interval_case(name, seed=71):
+    """one resident interval of INTERVAL_CASES[name]: random-phase coherencies whose cluster
+    amplitudes span three decades (cluster 0 the brightest), data = model at the true Jones plus noise
+    and 1 % outliers, NON-ZERO on flagged rows; random flag-1 and uv-cut (flag 2) rows, one station
+    (N > 2) and one timeslot (T > 1) fully flagged ("all-flagged": every row).  Jones points: A near
+    the truth (small residuals), B far from it, half: A with the first half of its values zeroed.
+    Coherencies are [row][M][4] complex, the data in API layout."""
+    N, M, T, nchunk = INTERVAL_CASES[name]
+    rng = np.random.default_rng(seed + 5 * N + M + T)
+    pr = synth.make_problem(N=N, M=M, tilesz=T, seed=seed + N, nchunk=nchunk, flag_frac=0.0,
+                            uvcut_frac=0.0, with_data=False)
+    R, Nb = pr.Nbase1, pr.Nbase
+    fl = np.zeros(R, dtype=np.uint8)
+    uu = rng.uniform(0, 1, R)
+    fl[uu < 0.06] = 1
+    fl[(uu >= 0.06) & (uu < 0.1)] = 2
+    if N > 2:
+        s = N // 2
+        fl[(pr.sta1 == s) | (pr.sta2 == s)] = 1
+    if T > 1:
+        t = T // 2
+        fl[t * Nb:(t + 1) * Nb] = 2
+    if name == "all-flagged":
+        fl[:] = 1
+    pr.flag = fl
+    amp = 10.0 ** -rng.uniform(0.0, 3.0, M)
+    amp[0] = 1.0
+    coh = np.empty((R, M, 4), dtype=np.complex128)
+    for k in range(M):
+        coh[:, k] = (amp[k] * rng.lognormal(0.0, 0.5, (R, 4))) * np.exp(2j * np.pi
+                                                                        * rng.uniform(0, 1, (R, 4)))
+    pr.coh = coh.reshape(-1)
+    x = synth.apply_jones(pr.coh, pr.jones_true, pr.sta1, pr.sta2, N, pr.nchunk)
+    sig = 1e-3 * np.median(np.abs(x))
+    x += rng.normal(0, sig, x.shape)
+    bad = rng.uniform(0, 1, x.shape) < 0.01
+    x[bad] += rng.normal(0, 50 * sig, int(bad.sum()))
+    pr.x = x
+    m = 8 * N * pr.Mt
+    A = pr.jones_true + 1e-4 * rng.normal(0, 1, m)
+    half = A.copy()
+    half[:m // 2] = 0.0
+    return dict(pr=pr, name=name, N=N, Nbase=Nb, tilesz=T, M=M, Mt=pr.Mt, nchunk=list(pr.nchunk),
+                sta1=pr.sta1, sta2=pr.sta2, flag=fl, coh=coh, x=x, m=m, amp=amp,
+                points=dict(A=A, B=pr.jones_true + 0.3 * rng.normal(0, 1, m), half=half))
+
+
+def _ld_scatter(idx, vals, n, cache, key, off=0):
+    """sums of the rows of vals [rows, 8] into n slots by off + idx, accumulated in long double; the
+    sort of idx is kept in cache[key] (one station map serves every cluster of one chunk count)"""
+    if key not in cache:
+        order = np.argsort(idx, kind="stable")
+        si = idx[order]
+        starts = np.flatnonzero(np.r_[True, si[1:] != si[:-1]])
+        cache[key] = (order, starts, si[starts])
+    order, starts, slots = cache[key]
+    out = np.zeros((n, vals.shape[1]), dtype=np.longdouble)
+    if len(order):
+        out[off + slots] = np.add.reduceat(vals[order], starts, axis=0, dtype=np.longdouble)
+    return out
+
+
+def interval_ref(case, p, nus=(None,), fault=None):
+    """plain per-row restatement of the full-interval passes, dirac_b200_predict (k_stream_all<0>) and
+    dirac_b200_grad (k_grad_tma_split), i.e. of the reference's minimize_viz_full_pth, cost_func /
+    robust_cost_func and grad_func / robust_grad_func (robust_lbfgs.c:424-560,155-316,674-735):
+      model     V = sum_k Jp C_k Jq^H, the chunk of a row by the row map (chunk_index, lmfit.c:655),
+                zero on every flagged row (flag 1 and uv-cut 2)
+      residual  e = x - V, every row (x itself on flagged rows)
+      cost      nu None: sum e^2 over every row and real component (flagged rows count with their
+                data); nu: sum log(1 + e e (1/nu)) (func_robust_th)
+      gradient  over the unflagged rows only, the chunk by the timeslot map (timeslot /
+                ceil(tilesz / nchunk), robust_lbfgs.c:197-207,465-475), with the reference's signs:
+                nu None  +2 sum Re(conj(e) dV/dtheta)      (-2 Re((f - x)^H df), :554)
+                nu       -2 sum psi(e) dV/dtheta, psi(e) = e / (nu + e^2) per real component (:299)
+    with the a-priori error budgets of any float64 evaluation of the same sums:
+      res_bound  (M + 10) u (|x| + sum_k |Jp||C_k||Jq|^T) per element (also bounds the model's error)
+      cost_bound rounding of each term, the residual error through d(term)/de, the summation
+      grad_bound per component: 2 (n u sum |psi(e)||dV/dtheta| + sum |psi'(e)| res_bound |dV/dtheta|),
+                 n = 8 (N - 1) T + 16
+    One cluster at a time; the sums are accumulated in long double.  `nus`: the gradients and costs to
+    take (None: Gaussian), all from the one model.  `fault` (one of INTERVAL_FAULTS) makes the
+    restatement deliberately wrong.  returns dict(model, res, res_bound, passes={nu: dict(cost,
+    cost_bound, grad, grad_bound)})"""
+    N, Nb, T, M = case["N"], case["Nbase"], case["tilesz"], case["M"]
+    R = Nb * T
+    u = U64
+    sta1, sta2 = case["sta1"], case["sta2"]
+    flagged = case["flag"] != 0
+    rows = np.arange(R)
+    tslot = rows // Nb
+    coh = case["coh"].reshape(R, M, 2, 2)
+    xc = _cplx(case["x"])
+    J = _jones(p, N * case["Mt"]).reshape(-1, N, 2, 2)
+    aJ = np.abs(J)
+    H = lambda X: np.conj(np.swapaxes(X, -1, -2))
+    Tt = lambda X: np.swapaxes(X, -1, -2)
+    c0 = np.concatenate([[0], np.cumsum(case["nchunk"])[:-1]]).astype(int)
+    rmap = lambda nch: synth.chunk_index(rows, R, nch)
+    tmap = lambda nch: tslot // (-(-T // nch))
+    # rows a faulty kernel would never visit: the last time block of the predict (2 timeslots) and of
+    # the gradient (4)
+    skip_m = np.zeros(R, dtype=bool)
+    skip_g = np.zeros(R, dtype=bool)
+    if fault == "drop_last_timeslot_block":
+        skip_m = tslot >= ((T - 1) // 2) * 2
+        skip_g = tslot >= ((T - 1) // 4) * 4
+
+    # a cluster whose Jones are all zero adds exactly nothing to the model and has a zero gradient
+    live = [J[c0[k]:c0[k] + case["nchunk"][k]].any() for k in range(M)]
+    V = np.zeros((R, 2, 2), dtype=np.clongdouble)
+    Va = np.zeros((R, 2, 2))
+    for k in range(M):
+        if (fault == "drop_third_warp" and k % 3 == 2) or not live[k]:
+            continue
+        cm = c0[k] + rmap(case["nchunk"][k])
+        C = np.ascontiguousarray(coh[:, k])
+        V += _mm2(_mm2(J[cm, sta1], C), H(J[cm, sta2]))
+        Va += _mm2(_mm2(aJ[cm, sta1], np.abs(C)), Tt(aJ[cm, sta2]))
+    V = V.astype(np.complex128)
+    V[flagged] = 0.0
+    Va[flagged] = 0.0
+    e = xc - V
+    e[skip_m] = 0.0
+    res = _api_layout(e)
+    res_bound = (M + 10) * u * np.repeat((np.abs(xc) + Va).reshape(-1), 2)
+    out = dict(model=_api_layout(V), res=res, res_bound=res_bound, passes={})
+
+    e8 = res.reshape(R, 8)
+    de8 = res_bound.reshape(R, 8)
+    keep = ~skip_m
+    use = ~skip_g if fault == "grad_over_flagged" else (~flagged & ~skip_g)
+    psis = {}
+    for nu in nus:
+        if nu is None:
+            terms = (e8 * e8)[keep]
+            cost_bound = (lsum(2 * u * terms) + lsum((2 * np.abs(e8) * de8 + de8 * de8)[keep])
+                          + terms.size * u * lsum(terms))
+            psi, dpsi = e8, de8
+        else:
+            terms = np.log(1.0 + e8 * e8 * (1.0 / nu))[keep]
+            cost_bound = (lsum(2 * u * (3.0 + terms)) + terms.size * u * lsum(terms)
+                          + lsum((2 * np.abs(e8) / (nu + e8 * e8) * de8)[keep]))
+            if fault == "robust_weight_complex":
+                a2 = np.repeat(e8[:, 0::2] ** 2 + e8[:, 1::2] ** 2, 2, axis=1)
+                psi = e8 / (nu + a2)
+            else:
+                psi = e8 / (nu + e8 * e8)
+            dpsi = np.abs((nu - e8 * e8) / (nu + e8 * e8) ** 2) * de8
+        psi = np.where(use[:, None], psi, 0.0)
+        dpsi = np.where(use[:, None], dpsi, 0.0)
+        W = (psi[:, 0::2] + 1j * psi[:, 1::2]).reshape(R, 2, 2)
+        Wa = (np.abs(psi[:, 0::2]) + np.abs(psi[:, 1::2])).reshape(R, 2, 2)
+        Wd = (dpsi[:, 0::2] + dpsi[:, 1::2]).reshape(R, 2, 2)
+        psis[nu] = (W, Wa, Wd)
+        out["passes"][nu] = dict(cost=lsum(terms), cost_bound=cost_bound)
+
+    nslot = case["Mt"] * N
+    nsum = 8 * max(N - 1, 1) * T + 16
+    G = {nu: np.zeros((nslot, 8), dtype=np.longdouble) for nu in nus}
+    Gb = {nu: np.zeros((nslot, 2, 2)) for nu in nus}
+    # which rows reach each end's sums: the faults that drop a kernel tile or a tile's last p
+    reach_p = np.ones(R, dtype=bool)
+    reach_q = np.ones(R, dtype=bool)
+    if fault == "drop_last_q_tile":
+        reach_p = reach_q = (sta2 // 32) != (N - 1) // 32
+    elif fault == "drop_last_p_of_tile":
+        reach_p = (sta1 % 8) != 7
+    cache = {}
+    for k in range(M):
+        if not live[k]:
+            continue
+        nch = case["nchunk"][k]
+        mk = "row" if fault == "grad_row_map" else "time"
+        lm = rmap(nch) if mk == "row" else tmap(nch)
+        gm = c0[k] + lm
+        kc = k - 2 if (fault == "stale_ring_stage" and k >= 2) else k
+        C = np.ascontiguousarray(coh[:, kc])
+        Ca = np.abs(C)
+        ip, iq = gm * N + sta1, gm * N + sta2
+        JqC = _mm2(J[gm, sta2], H(C))        # d/dJp of Re tr(W^H Jp C Jq^H): W Jq C^H
+        JpC = _mm2(J[gm, sta1], C)           # d/dJq: W^H Jp C
+        aJqC = _mm2(aJ[gm, sta2], Tt(Ca))
+        aJpC = _mm2(aJ[gm, sta1], Ca)
+        for nu in nus:
+            W, Wa, Wd = psis[nu]
+            vp = _split(_mm2(W, JqC)) * reach_p[:, None]
+            vq = _split(_mm2(H(W), JpC)) * reach_q[:, None]
+            G[nu] += _ld_scatter(lm * N + sta1, vp, nslot, cache, ("p", mk, nch), c0[k] * N)
+            G[nu] += _ld_scatter(lm * N + sta2, vq, nslot, cache, ("q", mk, nch), c0[k] * N)
+            Wb = nsum * u * Wa + Wd
+            Gb[nu] += _scatter2(ip, _mm2(Wb, aJqC), nslot)
+            Gb[nu] += _scatter2(iq, _mm2(Tt(Wb), aJpC), nslot)
+    for nu in nus:
+        sign = 2.0 if nu is None else -2.0
+        if fault == "grad_sign":
+            sign = -sign
+        out["passes"][nu]["grad"] = (sign * G[nu]).astype(np.float64).reshape(-1)
+        out["passes"][nu]["grad_bound"] = np.repeat((2.0 * Gb[nu]).reshape(-1), 2)
+    return out
